@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""bench.py — the hot path of BASELINE.json on B200: MultiGet lookups/s + replicated applies/s per GPU.
+"""bench.py — the hot path of BASELINE.json on H100: MultiGet lookups/s + replicated applies/s per GPU.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl b200|reference] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[1], SURVEY.md §8d "config 2"): 1024 shards on one GPU, 10 M KV total,
 16 B keys / 64 B values, loaded through the apply path and fully compacted.  One step =
@@ -12,6 +12,9 @@ stream); `applies` carries the apply-side numbers; `e2e` is the same through the
 (rsp_multi_get_fixed / rsp_apply_many) with pinned host memory, H2D + D2H inside the timed region.
 N > 1: one process per GPU (torchrun), each rank an independent engine with its own 1024 shards —
 shards partition shard_id -> GPU, no collective on the data path ("scaling": "weak").
+--dump-outputs DIR: after the timed steps, what the last step computed goes to DIR/*.npy (float32 / float64): a fixed,
+seeded sample of 65,536 of its MultiGet lookups (value bytes, lengths, statuses, key indices) and the per-batch statuses
+of its apply tick.  Inputs are seeded, so two builds can be compared output for output.
 """
 import argparse
 import ctypes as C
@@ -34,13 +37,13 @@ A_PUT = 83 + 22 + 88                     # per single-Put apply
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
-        return json.load(open(p)).get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+        return json.load(open(p)).get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json hbm_gbs)"
+    return 3350.0, "H100 SXM data sheet (HBM3, 3.35 TB/s)"
 
 
 def cpu_quota():
-    """CPUs of time the container may use per second (cgroup v2 cpu.max / v1 cfs quota); None when uncapped.  The GPU
-    boxes show 128 logical CPUs and cap the container at 16: every host-side figure is a figure under that quota."""
+    """CPUs of time the container may use per second (cgroup v2 cpu.max / v1 cfs quota); None when uncapped.  Every
+    host-side figure is a figure under that quota."""
     try:
         q, per = open("/sys/fs/cgroup/cpu.max").read().split()[:2]
         return None if q == "max" else float(q) / float(per)
@@ -104,7 +107,7 @@ class ClockSampler:
 def run_cpu(lib_kind, threads, shards, kv, apply_cap, get_secs, batch=4096, wal=1):
     """times oracle/okv_cpu_bench (the reference's RocksDB binary when oracle/_ref is present, else the port)"""
     from oracle import okv
-    okv.build(ref=os.path.isdir("/root/reference"))
+    okv.build(ref=False)
     lib = okv.REF_SO if (lib_kind == "reference" and okv.ref_available()) else okv.PORT_SO
     base = "/dev/shm" if os.path.isdir("/dev/shm") else "/tmp"
     d = os.path.join(base, "okv_bench_%d" % os.getpid())
@@ -183,6 +186,7 @@ def main():
     ap.add_argument("--cpu-get-secs", type=float, default=6.0)
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-seams", action="store_true", help="skip the through-the-seams phase (librsp_host.so)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/*.npy")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     local_rank = int(os.environ.get("LOCAL_RANK", "0"))
@@ -313,6 +317,13 @@ def main():
     want = synth.values(seed, (last % np.uint64(S)).astype(np.int64), last, 0)
     got = d_vals.cpu().numpy().reshape(Q, 64)
     assert np.array_equal(got, want), "MultiGet parity failed at full size"
+    dump = {}
+    if args.dump_outputs:
+        samp = np.sort(np.random.default_rng(0x5EED00D0).choice(Q, size=min(Q, 65536), replace=False))
+        dump = {"multiget_query": samp.astype(np.float64), "multiget_key_index": last[samp].astype(np.float64),
+                "multiget_value": got[samp].astype(np.float32),
+                "multiget_value_len": d_vlen.cpu().numpy()[samp].astype(np.float32),
+                "multiget_status": d_st.cpu().numpy()[samp].astype(np.float32)}
 
     # ---- config-2 variant: 10 % of the lookups ask for keys that were never written (NotFound) ------------
     with torch.cuda.stream(stream):
@@ -499,6 +510,8 @@ def main():
     fold()
     a_end.record(stream)
     assert bad_status == 0
+    if args.dump_outputs:
+        dump["apply_status"] = st_out.astype(np.float32)  # the last timed tick, one status per batch
     barrier()
     ap_total_ms = max_over_ranks(a_start.elapsed_time(a_end))
     ap_kernel_ms = eng.last_kernel_ms("apply")
@@ -776,17 +789,8 @@ def main():
     lookups_per_s = tot_lookups / (mg_total_ms * 1e-3)
     applies_per_s = tot_applies / (ap_total_ms * 1e-3)
     ach = A_GET * Q / (mg_kernel_ms * 1e-3) / 1e9
-    # DRAM traffic of the roofline kernel cannot be measured inside a timed run: it is what one `ncu --set full` capture of
-    # this same command recorded (dram__bytes_read.sum + dram__bytes_write.sum for one launch), kept under profiles/
-    traffic, traffic_src = None, None
-    tp = os.path.join(ROOT, "profiles", "multiget_traffic.json")
-    if os.path.exists(tp):
-        try:
-            tj = json.load(open(tp))
-            if tj.get("lookups_per_launch") == Q:
-                traffic, traffic_src = tj.get("dram_bytes_per_launch"), tj.get("source")
-        except Exception:
-            traffic = None
+    # DRAM traffic of the roofline kernel cannot be measured inside a timed run (it needs a hardware-counter profiler)
+    traffic, traffic_src = None, "not measured"
     # ---- the same path through the reference's seams: DbWrapper (pull loop) and ApplicationDB (MultiGet / Get) ------
     seams = None
     if not args.no_seams:
@@ -826,6 +830,10 @@ def main():
                "note": "the reference's options share one LRU block cache per DB among all reader threads; per-core figures are the fair comparison"}
     # (collectives are issued by every rank: none inside the rank-0 block below)
     big_applies_all = sum_over_ranks(big["batches_per_tick"] * big["ticks"]) if big else 0.0
+    if rank == 0 and args.dump_outputs:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, arr in dump.items():
+            np.save(os.path.join(args.dump_outputs, name + ".npy"), arr)
     if rank == 0:
         line = {
             "metric": "multiget_lookups_per_s", "value": lookups_per_s, "unit": "lookups/s", "n_gpus": world,

@@ -1,5 +1,5 @@
 /*
- * rsp_b200.h — the C ABI of librsp_b200.so: the drop-in boundary of the B200 engine.
+ * rsp_b200.h — the C ABI of librsp_b200.so: the drop-in boundary of the GPU engine.
  *
  * Everything the reference's hot path asks of RocksDB goes through these entry points; the C++
  * mirror of the reference interfaces (rocksplicator_b200/host/: rocksdb:: shim, replicator::DbWrapper

@@ -1,9 +1,10 @@
 """Generate tests/golden/*.json from the reference's OWN RocksDB binary (oracle/_ref).
 
-Run in the build container (needs oracle/_ref, i.e. /root/reference at build time):
+Run where oracle/_ref could be built (the reference's source tree at oracle/Makefile's REF):
     python -m oracle.gen_golden
-The fixtures pin the oracle port (tests/test_oracle_golden.py) and the CUDA engine (tests/test_parity_gpu.py)
-to outputs of the reference itself; they travel to the GPU box, /root/reference does not.
+The fixtures pin the oracle port (tests/test_oracle_golden.py, tests/test_sst_cpu.py) and the CUDA engine
+(tests/test_parity_gpu.py, tests/test_zz_ingest_gpu.py) to outputs of the reference itself, so that the tests need
+neither the reference nor its binary.
 TEST INFRASTRUCTURE ONLY.
 """
 import json
@@ -140,13 +141,164 @@ def gen_known_answers(ref):
     return rows
 
 
+LIVE_STREAMS = [(okv.MERGE_COUNTER, "counter", 91), (okv.MERGE_COUNTER, "counter", 92),
+                (okv.MERGE_APPEND, "append", 91), (okv.MERGE_APPEND, "append", 92)]
+FUZZ_SEEDS = range(200, 212)
+CORRUPT_FUZZ_SEEDS = range(0, 25)
+SST_READ_CASES = ((1, 11), (50, 12), (4000, 13))     # tests/test_sst_cpu.py: files the reference writes
+SST_INGEST_CASES = ((1, 21), (200, 22), (5000, 23))  # tests/test_sst_cpu.py: files written here, ingested by the reference
+
+
+def live_trace(lib, mop, mname, seed, flush):
+    """One random stream through one DB, then every read.  The reference's run flushes after batch 40 and compacts at
+    the end; the port's run does neither (its reads must not depend on where the data lives)."""
+    keys, stream = random_stream(seed + mop, 80, merge=mname)
+    db = okv.Okv(lib, merge_op=mop)
+    out = []
+    for i, (bt, ts) in enumerate(stream):
+        out.append(db.apply(bt, ts))
+        if flush and i == 40:
+            db.flush()
+    if flush:
+        db.compact()
+    out += [db.latest_seq(), [db.get(k) for k in keys], db.multi_get(keys), db.scan()]
+    db.close()
+    return out
+
+
+def sst_base(kv):
+    """what a reference-written SST file is delta-encoded against (tests/golden_util.py)"""
+    return b"".join(k + v for k, v in kv)
+
+
+def _ref_extras(ref_lib):
+    """the SST entry points of the driver over the reference's binary (oracle/ref_driver.c)"""
+    import ctypes as C
+    ref_lib.okv_write_sst.restype = C.c_int
+    ref_lib.okv_write_sst.argtypes = [C.c_char_p, C.c_size_t, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_char_p, C.c_size_t]
+    ref_lib.okv_ingest_sst.restype = C.c_int
+    ref_lib.okv_ingest_sst.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_char_p, C.c_size_t]
+    return ref_lib
+
+
+def gen_reference_runs(ref):
+    """The reference's side of the differential tests: fingerprints of what its binary returned (golden_util.digest),
+    and the SST files its SstFileWriter wrote (delta-encoded, tests/golden/ref_sst_<n>.delta)."""
+    import ctypes as C
+    import tempfile
+
+    import golden_util as G
+    from oracle.fuzz_corrupt_port_vs_ref import outcomes
+    from oracle.fuzz_port_vs_ref import trace
+    from rocksplicator_b200 import sst
+    from test_sst_cpu import _kv
+    out = {"live_streams": {"%s-%d" % (m, s): G.digest(live_trace(ref, mop, m, s, True)) for mop, m, s in LIVE_STREAMS}}
+    live_corrupt = []
+    for name, bt in corrupt_cases():
+        db = okv.Okv(ref, merge_op=okv.MERGE_UINT64ADD)
+        live_corrupt.append([name, db.apply(bt, 7), db.last_error, db.latest_seq()])
+        db.close()
+    out["live_corrupt"] = live_corrupt
+    out["fuzz"] = {str(s): G.digest(trace(ref, s)) for s in FUZZ_SEEDS}
+    out["corrupt_fuzz"] = {str(s): [[o[1], G.digest(o)] for o in outcomes(s, lambda mop: okv.Okv(ref, merge_op=mop))]
+                           for s in CORRUPT_FUZZ_SEEDS}
+    lib = _ref_extras(ref)
+    tmp = tempfile.mkdtemp()
+    out["sst_written_by_reference"] = {}
+    for n, seed in SST_READ_CASES:
+        kv = _kv(n, seed, max_v=2000)
+        koff = [0]
+        voff = [0]
+        for k, v in kv:
+            koff.append(koff[-1] + len(k))
+            voff.append(voff[-1] + len(v))
+        path = os.path.join(tmp, "ref%d.sst" % n)
+        err = C.create_string_buffer(256)
+        rc = lib.okv_write_sst(path.encode(), len(kv), b"".join(k for k, _ in kv) + b"\0", (C.c_uint64 * len(koff))(*koff),
+                               b"".join(v for _, v in kv) + b"\0", (C.c_uint64 * len(voff))(*voff), err, 256)
+        assert rc == 0, err.value
+        data = open(path, "rb").read()
+        delta = G.delta_encode(data, sst_base(kv))
+        assert G.delta_decode(delta, sst_base(kv)) == data
+        with open(os.path.join(OUT, "ref_sst_%d.delta" % n), "wb") as f:
+            f.write(delta)
+        out["sst_written_by_reference"][str(n)] = G.sha256(data)
+    out["sst_ingest"] = {}
+    for n, seed in SST_INGEST_CASES:
+        kv = _kv(n, seed, max_v=1500)
+        kv2 = [(k, b"second:" + v[:5]) for k, v in kv[::3]]
+        r = {}
+        db = okv.Okv(lib)
+        for tag, rows in (("", kv), ("2", kv2)):
+            data = sst.write_sst(rows)
+            path = os.path.join(tmp, "ours%d%s.sst" % (n, tag))
+            open(path, "wb").write(data)
+            err = C.create_string_buffer(256)
+            r["file" + tag] = G.sha256(data)
+            r["rc" + tag] = lib.okv_ingest_sst(db.h, path.encode(), 1, err, 256)
+            r["seq" + tag] = db.latest_seq()
+            r["scan" + tag] = G.digest(db.scan())
+            r["file%s_after" % tag] = G.sha256(open(path, "rb").read())
+            if not tag:
+                r["gets"] = G.digest([db.get(k) for k, _ in kv[:: max(1, len(kv) // 50)]])
+        db.close()
+        out["sst_ingest"][str(n)] = r
+    out["gpu_ingest"] = gen_ingest(lib, tmp)
+    return out
+
+
+def gen_ingest(lib, tmp):
+    """The reference's side of tests/test_zz_ingest_gpu.py::test_ingest_sequence_rules_and_contents, step for step:
+    ["ingest", file hash, allow, rc], ["apply", batch hash, rc], ["check", latest seq, contents fingerprint]."""
+    import ctypes as C
+
+    import golden_util as G
+    from rocksplicator_b200 import sst
+    from test_zz_ingest_gpu import _kv
+    db = okv.Okv(lib)
+    ev = []
+
+    def ingest(kv, allow=True):
+        data = sst.write_sst(kv)
+        path = os.path.join(tmp, "ingest%d.sst" % len(ev))
+        open(path, "wb").write(data)
+        err = C.create_string_buffer(256)
+        ev.append(["ingest", G.sha256(data), allow, lib.okv_ingest_sst(db.h, path.encode(), 1 if allow else 0, err, 256)])
+
+    def apply(data):
+        ev.append(["apply", G.sha256(data), db.apply(data, 1234)])
+
+    def check():
+        ev.append(["check", db.latest_seq(), G.digest(db.scan())])
+
+    f1 = _kv(3000, 1, lo=0, hi=1 << 20)
+    ingest(f1)
+    check()
+    apply(WriteBatch().put(f1[10][0], b"overwritten").delete(f1[11][0]).put(b"k-new", b"v").data())
+    check()
+    f2 = _kv(500, 2, lo=1 << 28, hi=1 << 29)
+    ingest(f2)
+    check()
+    f3 = sorted(dict([(k, b"third:" + v[:4]) for k, v in f1[::7]] + [(f1[11][0], b"back")]).items())
+    ingest(f3)
+    check()
+    ingest([(f1[5][0], b"refused")], allow=False)
+    check()
+    apply(WriteBatch().put(f3[0][0], b"after").delete(f2[0][0]).data())
+    check()
+    check()  # (after the engine's full compaction)
+    check()  # (after the engine refused two unsorted files)
+    db.close()
+    return ev
+
+
 def main():
     if not okv.ref_available():
-        raise SystemExit("oracle/_ref not built: run `make -C oracle ref` where /root/reference exists")
+        raise SystemExit("oracle/_ref not built: run `make -C oracle ref` with the reference's source tree at REF")
     ref = okv.load_ref()
     os.makedirs(OUT, exist_ok=True)
     for name, data in (("streams.json", gen_streams(ref)), ("corrupt.json", gen_corrupt(ref)),
-                       ("known_answers.json", gen_known_answers(ref))):
+                       ("known_answers.json", gen_known_answers(ref)), ("reference_runs.json", gen_reference_runs(ref))):
         with open(os.path.join(OUT, name), "w") as f:
             json.dump({"generator": "oracle/gen_golden.py", "source": "rocksdb_admin/tests/librocksdb.so.5.4",
                        "cases": data}, f, separators=(",", ":"))

@@ -19,7 +19,7 @@ MERGE_NONE, MERGE_COUNTER, MERGE_UINT64ADD, MERGE_APPEND = 0, 1, 2, 3
 
 
 def build(ref=True):
-    """Compile the checkers (gcc).  `ref` also (re)builds oracle/_ref when /root/reference exists."""
+    """Compile the checkers (gcc).  `ref` also (re)builds oracle/_ref when the reference's source tree is present."""
     subprocess.check_call(["make", "-s", "-C", HERE, "port", "bench"] + (["ref"] if ref else []),
                           stdout=subprocess.DEVNULL)
 

@@ -1,4 +1,4 @@
-"""rocksplicator_b200 — B200-native engine for Rocksplicator's sharded-replica hot path.
+"""rocksplicator_b200 — H100-native engine for Rocksplicator's sharded-replica hot path.
 
 Package contents: csrc/ (CUDA kernels + the C ABI of include/rsp_b200.h), host/ (C++ mirror of the
 reference's rocksdb:: / replicator:: / admin:: interfaces), engine.py (ctypes binding),

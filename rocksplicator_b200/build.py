@@ -1,8 +1,8 @@
-"""Builds librsp_b200.so (CUDA kernels + engine + C ABI) in-tree with nvcc for sm_100a.
+"""Builds librsp_b200.so (CUDA kernels + engine + C ABI) in-tree with nvcc for sm_90a (H100).
 
     python -m rocksplicator_b200.build [--force]
 
-The .so is git-ignored but travels to the GPU box with the gpurun snapshot.
+The .so and the objects under build/ are git-ignored build products.
 """
 import os
 import subprocess
@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "librsp_b200.so")
 SOURCES = ["k_apply.cu", "k_read.cu", "k_compact.cu", "engine.cu"]
 HEADERS = ["format.cuh", "kernels.h", "stager.h", "arena.h", os.path.join("..", "..", "include", "rsp_b200.h")]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall"] + os.environ.get("RSP_NVCC_EXTRA", "").split()
 
 
@@ -52,7 +52,7 @@ def build(force=False, verbose=False):
         list(ex.map(run, jobs))
     objs = [os.path.join(objdir, s.replace(".cu", ".o")) for s in SOURCES]
     if force or jobs or _stale(OUT, objs):
-        run([_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-o", OUT] + objs +
+        run([_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-o", OUT] + objs +
             ["-cudart", "static", "-lpthread", "-ldl", "-lrt"])
     return OUT
 

@@ -14,10 +14,9 @@ namespace rsp {
 
 // best-fit blocks with splitting and coalescing, carved from large slabs
 // Requests are rounded to 256 bytes and served from the smallest free block that fits (the remainder stays free); a
-// released block merges with its free neighbours inside its slab.  (r01 / early r02: power-of-two size classes with
-// per-class free lists.  A shard's runs grow from generation to generation, so the classes of the earlier generations
-// filled up with blocks nobody asked for again: the config-2 stretch point had 48 GB parked in free lists beside 125 GB
-// in use when the device ran out of memory — profiles/r02_stretch.md.)
+// released block merges with its free neighbours inside its slab.  (Power-of-two size classes with per-class free
+// lists do not work here: a shard's runs grow from generation to generation, so the classes of the earlier generations
+// fill up with blocks nobody asks for again.)
 struct Arena {
   std::mutex mu;
   size_t slab_bytes = 0;

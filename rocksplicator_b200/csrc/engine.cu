@@ -802,7 +802,7 @@ static void cut_chunks(GroupDesc* groups, size_t ng, Start start, End end, std::
 
 // Pitch of a batch in a staged image: whole 4-byte words, an ODD number of them — k_tick_fused walks a batch per thread
 // in shared memory, and equal-sized batches at an even word pitch (r02 padded to 16 bytes: 128 for the 115-byte
-// replication unit) put all 32 lanes of a warp on the same bank (ncu: 29.7-way conflicts, 97 % of the wavefronts).
+// replication unit) put all 32 lanes of a warp on the same bank.
 static inline size_t stage_pitch(size_t len_eff) {
   const size_t w = (len_eff + 3) / 4;
   return 4 * (w | 1);
@@ -1605,8 +1605,7 @@ static void iter_fetch(rsp_iter* it, const std::string* key, bool exclusive, boo
 // ------------------------------------------------------------------------------------------------
 // Asynchronous completions run here, not on a dispatcher thread (a dispatcher that runs user code cannot launch).
 // One task = ALL the completions of one device batch, run back to back by one thread: a wake-up per batch, not per
-// response (the box's CPU time is capped: a thread hand-off per response was most of the follower's cost,
-// profiles/r02_seams_trace.md); a large batch is split over a few threads, eight completions or more each.
+// response (a thread hand-off per response costs CPU time the follower's data path needs); a large batch is split over a few threads, eight completions or more each.
 struct CompletionPool {
   std::mutex mu;
   std::condition_variable cv;
@@ -1992,7 +1991,7 @@ static int apply_combined(rsp_shard* s, size_t n, const rsp_slice* batches, cons
 // ------------------------------------------------------------------------------------------------
 extern "C" {
 
-const char* rsp_version(void) { return "rocksplicator_b200 0.1 (sm_100a)"; }
+const char* rsp_version(void) { return "rocksplicator_b200 0.1 (sm_90a)"; }
 
 int rsp_engine_create(int device, const rsp_engine_cfg* cfg, rsp_engine** out) {
   try {
@@ -2019,7 +2018,7 @@ int rsp_engine_create(int device, const rsp_engine_cfg* cfg, rsp_engine** out) {
   e->arena.slab_bytes = e->cfg.arena_bytes;
   e->arena.slab_alloc = arena_slab_alloc;
   e->arena.slab_free = arena_slab_free;
-  // measured on the B200 host (128 cores): 2 staging threads 29 M applies/s, 1: 27, 8: 19 (spawn cost wins)
+  // two staging threads: more cost more in thread spawns than they save in copies
   e->stage_threads = 2;
   if (const char* t = getenv("RSP_STAGE_THREADS")) e->stage_threads = (size_t)std::max(1, atoi(t));
   if (const char* t = getenv("RSP_FUSED_TICK")) e->fused_ticks = atoi(t) != 0;

@@ -738,7 +738,7 @@ __global__ void __launch_bounds__(TC_THREADS, 8) k_tick_chunks(FusedTick t, Shar
   const u32 first_bad = s_first_bad;
   // ---- the predecessor's record, AFTER this chunk's own decode: a chunk that waits has nothing left to do but the
   // totals, so the chain advances in a few hundred nanoseconds per link (polling before the decode serialised the
-  // decodes of a group: 250 us per 1 M-batch tick instead of the 186 us of the CTA-per-group kernel)
+  // decodes of a group, slower than the CTA-per-group kernel)
   if (tid == 0) {
     u64 seq; u32 tail, cnt, latch, flags = 0;
     if (ck.index_in_group == 0) {
@@ -846,11 +846,11 @@ void launch_tick_fused(const FusedTick& t, ShardDev* shards, ShardFast* fast, u3
     k_tick_fused<64, 16><<<t.n_groups, 64, 0, s>>>(t, shards, fast, mt_filter);
   } else {
     // Long groups: a CTA per group (k_tick_fused at 128 threads, the chunks of a group one after the other) when the
-    // groups alone fill the machine, a CTA per chunk (k_tick_chunks) when they do not — measured on 1024 groups x 1000
-    // batches: 198 us per group vs 233 us per chunk (the chain of a group costs more than the tail of one wave,
-    // profiles/r02_tick_ab.md); a tick of a few very long groups has no other source of parallelism than its chunks.
+    // groups alone fill the machine, a CTA per chunk (k_tick_chunks) when they do not — with enough groups the chain
+    // of a group costs more than the tail of one wave; a tick of a few very long groups has no other source of
+    // parallelism than its chunks.
     static const int force = [] { const char* v = getenv("RSP_TICK_CHUNKS"); return v ? (atoi(v) ? 1 : 0) : -1; }();
-    const bool per_group = force < 0 ? t.n_groups >= 4u * 148u : force == 0;
+    const bool per_group = force < 0 ? t.n_groups >= 4u * DEVICE_SMS : force == 0;
     if (per_group) {
       k_tick_fused<128, 8><<<t.n_groups, 128, 0, s>>>(t, shards, fast, mt_filter);
       return;

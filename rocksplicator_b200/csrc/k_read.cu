@@ -268,9 +268,8 @@ __global__ void __launch_bounds__(256) k_multi_get(GetArgs a) {
   lookup_generic(a, q, lane, gmask, gbase);
 }
 
-// Measured and dropped in r02 (profiles/r02_experiments/): hash-addressed entry slots instead of the index
-// (0.38 / 0.32 / 0.18 of the roofline at load 0.25 / 0.5 / 0.75 against 0.41) and software prefetch of later lookups'
-// sectors (0.18).
+// Tried and dropped: hash-addressed entry slots instead of the index, and software prefetch of later lookups' sectors
+// (both slower than the index probe below).
 // ---- the hot kernel: 16-byte keys, TWO lanes per lookup, three dependent memory round trips ----------
 //   1. shard id + query key (coalesced across the warp) and the 32-byte ShardFast descriptor
 //      (32 B x #shards: L1/L2-resident); both lanes load the same words (one broadcast transaction)
@@ -289,9 +288,8 @@ static_assert(sizeof(ShardFast) == 32, "ShardFast");
 constexpr u32 FL = 2;  // lanes per lookup
 
 // L2 residency control (createpolicy + ld/st .L2::cache_hint): the hash-index sectors are the only
-// data with reuse across lookups (80 MB at 10 M keys vs a 126 MB L2); entries, query keys and results
-// stream through once.  RSP_MG_HINTS: 0 = none, 1 = index evict_last (+1 %), 2 = also streams evict_first
-// (measured 20 % SLOWER on B200: kept only as an experiment switch).  RSP_MG_NOALLOC: entry units bypass L1.
+// data with reuse across lookups (80 MB at 10 M keys against a 50 MB L2); entries, query keys and results stream through once.  RSP_MG_HINTS: 0 = none, 1 = index evict_last, 2 = also
+// streams evict_first (an experiment switch).  RSP_MG_NOALLOC: entry units bypass L1.
 #ifndef RSP_MG_HINTS
 #define RSP_MG_HINTS 1
 #endif
@@ -343,7 +341,7 @@ __device__ __forceinline__ void stg_pol(uint4* p, const uint4& v, u64 pol) {
 // Candidate entry at `ent`: header unit 0, key unit KU, value units KU+1.. (U units in all).
 // Returns 0 = served, 1 = not my key (tag false positive), 2 = needs the generic path.
 #ifndef RSP_MG_NOALLOC
-#define RSP_MG_NOALLOC 0  // measured 5 % slower with L1::no_allocate on the entry units
+#define RSP_MG_NOALLOC 0  // L1::no_allocate on the entry units (an experiment switch)
 #endif
 #ifndef RSP_MG_MEMSET
 #define RSP_MG_MEMSET 1
@@ -531,8 +529,7 @@ __global__ void __launch_bounds__(RSP_MG_TPB, RSP_MG_MINB) k_multi_get16(GetArgs
     }
   }
   // this launch counts in n_pending[parity].  Clearing the other counter here instead of a memset node
-  // before the launch measured 20 % SLOWER end to end on B200 (14.98 -> 12.08 G lookups/s), so the
-  // memset node stays (RSP_MG_MEMSET=1).
+  // before the launch was slower end to end, so the memset node stays (RSP_MG_MEMSET=1).
 #if !RSP_MG_MEMSET
   if (blockIdx.x == 0 && threadIdx.x == 0) a.n_pending[a.parity ^ 1u] = 0;
 #endif
@@ -625,9 +622,8 @@ __device__ __forceinline__ u32 probe_one_run(const uint4& g0, const uint4& g1, c
 
 // k_multi_get16m: the same lookup for engines where some shard has SEVERAL sorted runs (between a flush and the next
 // merge): the runs are walked newest first, a run that does not hold the key hands over to the next older one
-// (per-run descriptors behind the ShardFast array).  The single-run kernel above is kept exactly as measured in r01:
-// folding both into one template cost it 20 % (13.3 instead of 16.2 G lookups/s on the same B200, same instruction
-// mix — profiles/r02_regression_bisect.md), so the host picks the kernel per launch instead.
+// (per-run descriptors behind the ShardFast array).  The single-run kernel above is kept on its own: folding both into
+// one template changes its register allocation at the same instruction mix, so the host picks the kernel per launch.
 template <bool BIG>
 __global__ void __launch_bounds__(RSP_MG_TPB, RSP_MG_MINB) k_multi_get16m(GetArgs a) {
   constexpr bool MULTI = true;
@@ -741,7 +737,7 @@ void launch_multi_get(const GetArgs& a, cudaStream_t s) {
     } else {
       if (multi) k_multi_get16m<false><<<g16, RSP_MG_TPB, 0, s>>>(a); else k_multi_get16<false><<<g16, RSP_MG_TPB, 0, s>>>(a);
     }
-    k_multi_get_pending<<<std::min<u32>(grid, 148u), 256, 0, s>>>(a);
+    k_multi_get_pending<<<std::min<u32>(grid, DEVICE_SMS), 256, 0, s>>>(a);
   } else {
     k_multi_get<<<grid, 256, 0, s>>>(a);
   }
@@ -856,7 +852,7 @@ __device__ __forceinline__ void warp_copy_bytes(u8* dst, const u8* src, u32 n, u
 // counts prefixes below / not above the target 32 at a time with ballots, and resolves the final position
 // inside the 1-2 candidate blocks by comparing 32 entry keys at once.
 // independent loads per lane in the streaming loop: 4 gives 181 M scans/s, the plain loop (one load in flight per
-// warp: LDG, STG, LDG, ...) 115 M (profiles/r02_experiments/)
+// warp: LDG, STG, LDG, ...) leaves the load latency exposed
 #define RSP_SCAN_UNROLL 4
 constexpr u32 SCAN_WARPS = 4;
 constexpr u32 SCAN_STAGE_PFX = 512;  // prefixes staged per warp (4 KB): runs up to 16 K entries

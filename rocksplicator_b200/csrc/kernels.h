@@ -4,6 +4,9 @@
 
 namespace rsp {
 
+// SMs of the target GPU (H100 SXM): sizes the grids that should fill the machine exactly once
+constexpr u32 DEVICE_SMS = 132;
+
 // ---- apply tick image (device) -------------------------------------------------------------------
 struct BatchDesc {
   u32 shard_ix;
@@ -137,8 +140,8 @@ struct GetArgs {
   u32 max_shards;        // shard ids >= this answer InvalidArgument
   u32 multirun;          // some live shard has more than one run: k_multi_get16m walks the runs newest first; the per-run
                          // descriptors ([max_shards][RSP_MAX_RUNS]) follow the ShardFast array in the same allocation.
-                         // (The struct keeps its r01 size and field offsets: growing it by eight bytes changes the
-                         // register allocation of k_multi_get16 and costs it 20 % — profiles/r02_regression_bisect.md)
+                         // (The struct keeps its size and field offsets: growing it by eight bytes changes the
+                         // register allocation of k_multi_get16 and slows it down)
 };
 static_assert(sizeof(GetArgs) == 128, "GetArgs layout is part of k_multi_get16's measured code generation");
 void launch_multi_get(const GetArgs& a, cudaStream_t s);

@@ -19,8 +19,8 @@
 //
 // Synchronisation.  The OPEN batch is one 64-bit word — buffer | class | items reserved | bytes reserved — and a
 // reservation is one compare-and-swap on it: hundreds of callers arriving together (every caller of a batch comes back
-// at the same moment) do not queue on a lock.  (With the reservation under the spin lock, 256 Get callers spent 135 us
-// of CPU time per Get, most of it spinning for that lock, against 20 us at 64 callers: profiles/r02_seams_trace.md.)
+// at the same moment) do not queue on a lock.  (With the reservation under the spin lock, hundreds of Get callers spent
+// most of their CPU time spinning for that lock.)
 // Only the transitions of a BUFFER (close, open, free) take the spin lock, and only the dispatcher and the last
 // caller out of a batch make them.  The dispatcher knows a closed batch is complete when the items committed equal the
 // items reserved, and a buffer is free again when the items released do.

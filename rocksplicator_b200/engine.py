@@ -1,6 +1,6 @@
 """ctypes binding of librsp_b200.so (include/rsp_b200.h): the product's Python face.
 
-There is no CPU path behind these classes: if the CUDA library is missing or no B200 is visible the
+There is no CPU path behind these classes: if the CUDA library is missing or no GPU is visible the
 constructors raise.  Method names on `Shard` follow the reference's rocksdb::DB / DbWrapper usage
 (rocksdb_replicator/rocksdb_wrapper.cpp, rocksdb_admin/application_db.cpp).
 """

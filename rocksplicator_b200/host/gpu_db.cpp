@@ -45,7 +45,7 @@ int GpuDB::MergeTrampoline(void* state, const uint8_t* key, size_t klen, const u
 Status GpuDB::Open(const rocksdb::Options& options, const std::string& name, rocksdb::DB** dbptr, int device) {
   *dbptr = nullptr;
   auto engine = GpuEngine::ForDevice(device);
-  if (!engine) return Status::IOError("no usable CUDA device for the B200 engine (there is no CPU fallback)");
+  if (!engine) return Status::IOError("no usable CUDA device for the GPU engine (there is no CPU fallback)");
   rsp_shard_opts so;
   memset(&so, 0, sizeof(so));
   so.write_buffer_bytes = options.write_buffer_size;

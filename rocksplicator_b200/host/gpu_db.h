@@ -1,4 +1,4 @@
-// gpu_db.h — rocksdb::DB over the B200 engine's C ABI (include/rsp_b200.h).  This is the object handed to
+// gpu_db.h — rocksdb::DB over the GPU engine's C ABI (include/rsp_b200.h).  This is the object handed to
 // RocksDBReplicator::addDB / ApplicationDB in place of the rocksdb::DB* that rocksdb::DB::Open returns at
 // rocksdb_admin/admin_handler.cpp:640.  Host code only: no CUDA types; every data call ends in librsp_b200.so.
 #pragma once
@@ -99,8 +99,8 @@ class GpuDB : public rocksdb::DB {
                              void* out_ctx);
   // One chunk of the update log = what ONE call appended (a leader's Write: one batch; a follower's response: its <= 50
   // updates), the batches back to back in one string: three allocations per response instead of two per update — with
-  // a std::string + shared_ptr per update the completion threads spent 170 us per response in malloc / free
-  // (profiles/r02_seams_trace.md) and bounded the whole pull loop.
+  // a std::string + shared_ptr per update the completion threads spent their time in malloc / free and bounded the
+  // whole pull loop.
   struct LogChunk {
     struct Rec { uint32_t off, len, count; rocksdb::SequenceNumber first_seq; };
     rocksdb::SequenceNumber first_seq = 0, last_seq = 0;

@@ -1,5 +1,5 @@
 // rocksdb/db.h — the rocksdb::DB surface ApplicationDB and RocksDbWrapper call
-// (rocksdb_admin/application_db.cpp:78-225, rocksdb_replicator/rocksdb_wrapper.cpp:4-28).  The B200
+// (rocksdb_admin/application_db.cpp:78-225, rocksdb_replicator/rocksdb_wrapper.cpp:4-28).  The GPU
 // implementation is gpu_db.h's GpuDB; members the hot path never reaches answer NotSupported.
 #pragma once
 #include <map>

@@ -1,5 +1,5 @@
 // rocksdb/options.h — option structs named by the reference's call sites.  Only the fields the hot path
-// reads are honoured by the B200 engine (write_buffer_size, merge_operator, level0 trigger).
+// reads are honoured by the GPU engine (write_buffer_size, merge_operator, level0 trigger).
 #pragma once
 #include <cstdint>
 #include <memory>

@@ -2,7 +2,7 @@
 //
 // Interface parity target: replicator::DbWrapper in the reference (rocksdb_replicator/db_wrapper.h:6-15) — the same
 // four operations with the same argument meaning, so that a wrapper written against one compiles against the other.
-// Implementations: GpuDbWrapper (gpu_db_wrapper.h, the B200 engine); in the reference RocksDbWrapper
+// Implementations: GpuDbWrapper (gpu_db_wrapper.h, the GPU engine); in the reference RocksDbWrapper
 // (rocksdb_wrapper.cpp), the CDC observer (cdc_admin/cdc_application_db.cpp:19-37) and TestDBProxy.
 #pragma once
 #include <cstdint>
@@ -36,7 +36,7 @@ class DbWrapper {
   // applied; the pull loop backs off and asks for the same sequence again.
   virtual bool HandleReplicateResponse(Update* update) = 0;
 
-  // FOLLOWER side, B200 addition (not in the reference's interface; the default keeps every existing wrapper valid):
+  // FOLLOWER side, GPU-engine addition (not in the reference's interface; the default keeps every existing wrapper valid):
   // apply the updates of ONE ReplicateResponse in order and report how many were applied — the body of the
   // reference's hot loop (replicated_db.cpp:369-383: one HandleReplicateResponse per update, stop at the first
   // failure).  done may run later on another thread; `updates` must stay alive until then.  A wrapper whose store

@@ -38,8 +38,7 @@ class Executor {
     }
     const int64_t queued = queued_.fetch_add(1, std::memory_order_acq_rel) + 1;
     // Wake a worker only when the ones already awake will not get to the task soon: a wake-up and the sleep after it
-    // cost more CPU time than a short task, and the GPU boxes cap the container's CPU time (profiles/
-    // r02_seams_trace.md).  An awake worker drains its own queue and steals from the others before it sleeps.
+    // cost more CPU time than a short task, and a container's CPU time may be capped.  An awake worker drains its own queue and steals from the others before it sleeps.
     const int64_t awake = (int64_t)n_ - sleepers_.load(std::memory_order_acquire);
     if (awake <= 0 || queued > 2 * awake) {
       if (q.sleeping.load(std::memory_order_acquire)) q.cv.notify_one();

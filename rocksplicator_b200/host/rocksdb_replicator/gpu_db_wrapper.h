@@ -1,4 +1,4 @@
-// gpu_db_wrapper.h — replicator::DbWrapper over the B200 engine: the drop-in for RocksDbWrapper
+// gpu_db_wrapper.h — replicator::DbWrapper over the GPU engine: the drop-in for RocksDbWrapper
 // (rocksdb_replicator/rocksdb_wrapper.{h,cpp}).  Same four methods, same meaning.
 #pragma once
 #include <memory>

@@ -367,7 +367,7 @@ RocksDBReplicator::~RocksDBReplicator() {
 
 ReturnCode RocksDBReplicator::addDB(const std::string& db_name, std::shared_ptr<rocksdb::DB> db, ReplicaRole role,
                                     const SocketAddress& upstream_addr, ReplicatedDB** replicated_db) {
-  // rocksdb_replicator.cpp:96-105 wraps the DB in RocksDbWrapper; here the wrapper is the B200 one
+  // rocksdb_replicator.cpp:96-105 wraps the DB in RocksDbWrapper; here the wrapper is the GPU one
   return addDB(db_name, std::static_pointer_cast<DbWrapper>(std::make_shared<GpuDbWrapper>(db_name, std::move(db))), role,
                upstream_addr, replicated_db);
 }

@@ -2,7 +2,7 @@
 // (rocksdb_replicator/rocksdb_replicator.h:71-216): addDB (two overloads), removeDB, write,
 // ReplicatedDB::Write / Introspect, ReturnCode, LogExtractor.  The replication protocol logic (pull loop,
 // long-poll serving, ACK modes, upstream reset hook) follows rocksdb_replicator/replicated_db.cpp; the
-// storage below the DbWrapper seam is the B200 engine.
+// storage below the DbWrapper seam is the GPU engine.
 #pragma once
 #include <atomic>
 #include <list>

@@ -457,7 +457,7 @@ static void test_dbconfig_and_stats() {
   fast_flags();
 }
 
-// ---- GPU-backed: the DB below the seam is the B200 engine -----------------------------------------------
+// ---- GPU-backed: the DB below the seam is the GPU engine -----------------------------------------------
 class CounterMergeOperator : public rocksdb::AssociativeMergeOperator {  // examples/counter_service/merge_operator.cpp
  public:
   bool Merge(const Slice&, const Slice* existing, const Slice& value, std::string* nv, rocksdb::Logger*) const override {

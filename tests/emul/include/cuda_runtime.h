@@ -6,7 +6,7 @@
 // inline-PTX helpers (cache-policy loads, the TMA bulk copy + mbarrier) and the dynamic shared-memory declaration: nvcc
 // never defines RSP_EMUL, and tools/sass_identity.py shows the kernels' SASS is unchanged by them.  The emulation says
 // nothing about performance and nothing about memory-model races — every parity claim is made by the `-m gpu` tests
-// on a B200.
+// on an H100.
 //
 // Execution model: a launch runs synchronously in the calling thread, block after block.  Every CUDA thread of a
 // block is a fiber (ucontext); fibers run until they reach a warp collective (__shfl*_sync, __ballot_sync,

@@ -1,7 +1,7 @@
 """Out-of-device-memory behaviour on the emulation (RSP_EMUL_DEVICE_BYTES caps the emulated device): applies are refused
 with an IO error once the device is full, nothing that was acknowledged is lost or changed, closing shards gives memory
-back and applies go on.  Run by tests/test_emul_cpu.py; no GPU equivalent (a B200 that is driven out of memory under
-gpurun counts as a strike)."""
+back and applies go on.  Run by tests/test_emul_cpu.py; no GPU equivalent (a GPU shared with other work is not driven
+out of memory on purpose)."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))
 sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__)))))

@@ -45,7 +45,7 @@ def test_product_does_not_touch_oracle():
 
 
 def test_product_library_has_no_emulation_or_cpu_path():
-    """librsp_b200.so is the nvcc build: none of tests/emul's symbols, device code for sm_100a inside, and the Python
+    """librsp_b200.so is the nvcc build: none of tests/emul's symbols, device code for sm_90a inside, and the Python
     binding names no other library.  (tests/emul builds a separate test-only library from the same sources.)"""
     import subprocess
     from rocksplicator_b200 import engine
@@ -55,7 +55,7 @@ def test_product_library_has_no_emulation_or_cpu_path():
     assert "emul_launch" not in syms and "emul_collective" not in syms
     elf = subprocess.run(["cuobjdump", "-lelf", so], capture_output=True, text=True)
     if elf.returncode == 0:  # cuobjdump ships with the CUDA toolkit
-        assert "sm_100a" in elf.stdout, elf.stdout[:300]
+        assert "sm_90a" in elf.stdout, elf.stdout[:300]
     for dp, _, fs in os.walk(os.path.join(ROOT, "rocksplicator_b200")):
         for f in fs:
             if f.endswith(".py"):

@@ -5,7 +5,7 @@ re-run against that build in a subprocess.
 
 What this is for: catching logic and addressing bugs before GPU time is spent (tests/emul/build_emul.py --asan runs
 the same under AddressSanitizer).  What it is NOT: a product path, a fallback, or a parity claim — librsp_b200.so is
-CUDA-only and the parity tests proper are the `-m gpu` runs on a B200.
+CUDA-only and the parity tests proper are the `-m gpu` runs on an H100.
 """
 import importlib.util
 import os
@@ -114,7 +114,7 @@ def test_host_mirror_over_emulated_engine(emul):
 def test_out_of_device_memory_paths(emul):
     """tests/emul/oom_probe.py with the emulated device capped at 8 MB: once the device is full applies are refused with an
     IO error (the flush that would make room cannot allocate), everything acknowledged before stays readable bit for bit,
-    and applies go on after shards were closed.  (No GPU twin: driving a B200 out of memory under gpurun is a strike.)"""
+    and applies go on after shards were closed.  (No GPU twin: a GPU shared with other work is not driven out of memory on purpose.)"""
     env = dict(os.environ)
     env.update({"RSP_TEST_EMUL_LIB": emul[0], "RSP_EMUL_DEVICE_BYTES": str(8 << 20)})
     p = subprocess.run([sys.executable, os.path.join(ROOT, "tests", "emul", "oom_probe.py")], cwd=ROOT, env=env,

@@ -1,7 +1,8 @@
 """Pins the oracle port (oracle/kv_oracle.c) to the reference:
   1. known-answer table measured on the reference's shipped librocksdb.so.5.4 (SURVEY.md §9),
   2. tests/golden/*.json generated from that binary by oracle/gen_golden.py,
-  3. live differential runs against the binary when oracle/_ref is present (build container).
+  3. differential runs (random streams, fuzzed streams, mutated batches) against the binary's results on the same
+     inputs, stored in tests/golden/reference_runs.json.
 CPU only.
 """
 import struct
@@ -111,52 +112,43 @@ def test_replicator_test_vectors(port_lib):
     db.close()
 
 
-def test_port_vs_reference_live(port_lib, ref_lib):
-    """Differential: fresh random streams (not in the fixtures) through both."""
-    for mop, mname in ((okv.MERGE_COUNTER, "counter"), (okv.MERGE_APPEND, "append")):
-        for seed in (91, 92):
-            keys, stream = random_stream(seed + mop, 80, merge=mname)
-            a = okv.Okv(port_lib, merge_op=mop)
-            b = okv.Okv(ref_lib, merge_op=mop)
-            for i, (bt, ts) in enumerate(stream):
-                assert a.apply(bt, ts) == b.apply(bt, ts)
-                if i == 40:
-                    b.flush()
-            b.compact()
-            assert a.latest_seq() == b.latest_seq()
-            for k in keys:
-                assert a.get(k) == b.get(k)
-            assert a.multi_get(keys) == b.multi_get(keys)
-            assert a.scan() == b.scan()
-            a.close()
-            b.close()
-    for name, bt in corrupt_cases():
+def test_port_vs_reference_live(port_lib):
+    """Differential: fresh random streams (not in the stream fixtures) through the port, against what the reference's
+    binary returned for the same streams (tests/golden/reference_runs.json, oracle/gen_golden.py)."""
+    from oracle import gen_golden
+    want = G.load("reference_runs.json")
+    for mop, mname, seed in gen_golden.LIVE_STREAMS:
+        got = gen_golden.live_trace(port_lib, mop, mname, seed, flush=False)
+        assert G.digest(got) == want["live_streams"]["%s-%d" % (mname, seed)], (mname, seed)
+    cases = corrupt_cases()
+    assert [name for name, _ in cases] == [w[0] for w in want["live_corrupt"]]
+    for (name, bt), w in zip(cases, want["live_corrupt"]):
         a = okv.Okv(port_lib, merge_op=okv.MERGE_UINT64ADD)
-        b = okv.Okv(ref_lib, merge_op=okv.MERGE_UINT64ADD)
-        assert a.apply(bt, 7) == b.apply(bt, 7), name
-        assert a.last_error == b.last_error, name
-        assert a.latest_seq() == b.latest_seq(), name
+        assert [name, a.apply(bt, 7), a.last_error, a.latest_seq()] == w, name
         a.close()
-        b.close()
 
 
-def test_port_vs_reference_fuzz(port_lib, ref_lib):
-    """oracle/fuzz_port_vs_ref.py on a few seeds: flush/compaction at random points, MultiGet, iterator walks."""
-    import importlib.util
-    import os
-    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "fuzz_port_vs_ref.py")
-    spec = importlib.util.spec_from_file_location("fuzz_port_vs_ref", path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    assert mod.run(200, 212, port_lib, ref_lib) == 0
+def test_port_vs_reference_fuzz(port_lib):
+    """oracle/fuzz_port_vs_ref.py on a few seeds: flush/compaction at random points, MultiGet, iterator walks; the
+    reference's traces of the same seeds are stored as fingerprints."""
+    from oracle import fuzz_port_vs_ref, gen_golden
+    want = G.load("reference_runs.json")["fuzz"]
+    assert sorted(int(s) for s in want) == list(gen_golden.FUZZ_SEEDS)
+    diverged = [s for s in gen_golden.FUZZ_SEEDS if G.digest(fuzz_port_vs_ref.trace(port_lib, s)) != want[str(s)]]
+    assert not diverged, diverged
 
 
-def test_port_vs_reference_corruption_fuzz(port_lib, ref_lib):
+def test_port_vs_reference_corruption_fuzz(port_lib):
     """oracle/fuzz_corrupt_port_vs_ref.py on a few seeds: mutated batches, error class + text + latch + contents"""
-    import importlib.util
-    import os
-    path = os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle", "fuzz_corrupt_port_vs_ref.py")
-    spec = importlib.util.spec_from_file_location("fuzz_corrupt_port_vs_ref", path)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    assert mod.run(0, 25, port_lib, ref_lib) == 0
+    from oracle import fuzz_corrupt_port_vs_ref as fz
+    from oracle import gen_golden
+    want = G.load("reference_runs.json")["corrupt_fuzz"]
+    assert sorted(int(s) for s in want) == list(gen_golden.CORRUPT_FUZZ_SEEDS)
+    bad = []
+    for seed in gen_golden.CORRUPT_FUZZ_SEEDS:
+        got = fz.outcomes(seed, lambda mop: okv.Okv(port_lib, merge_op=mop))
+        assert len(got) == len(want[str(seed)])
+        for i, (ra, (rb_rc, rb_digest)) in enumerate(zip(got, want[str(seed)])):
+            if G.digest(ra) != rb_digest and not fz.is_known_deviation(ra, rb_rc):
+                bad.append((seed, i, ra[1], rb_rc, ra[2]))
+    assert not bad, bad[:5]

@@ -1,16 +1,17 @@
 """SST interchange on the host (SURVEY §8f rank 2), CPU only.
   * the reference's golden file rocksdb_admin/tests/old_sst_data.sst (copied byte-for-byte to tests/golden/: a 978-byte
     test fixture, Snappy-compressed block) must read as key0..key9 -> value0..value9 (sst_binary.cpp:43-58);
-  * files written by the reference's own SstFileWriter (librocksdb.so.5.4) must read back exactly;
-  * files written by OUR writer must be accepted by the reference's DB::IngestExternalFile and scan back exactly,
+  * files written by the reference's own SstFileWriter (librocksdb.so.5.4, stored under tests/golden/) must read back
+    exactly;
+  * files written by OUR writer must be those the reference's DB::IngestExternalFile accepted and scanned back exactly,
     with the sequence-number rule of rocksdb_assumption_test.cpp:248-262 (ingest into an empty DB: seq stays 0)."""
-import ctypes as C
 import os
 import random
 import tempfile
 
 import pytest
 
+import golden_util as G
 from rocksplicator_b200 import sst
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "old_sst_data.sst")
@@ -48,63 +49,45 @@ def test_roundtrip_own_writer_reader():
         sst.write_sst([(b"b", b"1"), (b"a", b"2")])  # "Keys must be added in order"
 
 
-def _ref_extras(ref_lib):
-    ref_lib.okv_write_sst.restype = C.c_int
-    ref_lib.okv_write_sst.argtypes = [C.c_char_p, C.c_size_t, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_char_p, C.c_size_t]
-    ref_lib.okv_ingest_sst.restype = C.c_int
-    ref_lib.okv_ingest_sst.argtypes = [C.c_void_p, C.c_char_p, C.c_int, C.c_char_p, C.c_size_t]
-    return ref_lib
-
-
-def test_reads_files_written_by_the_reference(ref_lib):
-    import numpy as np
-    lib = _ref_extras(ref_lib)
-    tmp = tempfile.mkdtemp(dir="/dev/shm" if os.path.isdir("/dev/shm") else None)
-    for n, seed in ((1, 11), (50, 12), (4000, 13)):
+def test_reads_files_written_by_the_reference():
+    """files the reference's SstFileWriter wrote for these key / value sets, stored as deltas against the sets"""
+    from oracle import gen_golden
+    want = G.load("reference_runs.json")["sst_written_by_reference"]
+    for n, seed in gen_golden.SST_READ_CASES:
         kv = _kv(n, seed, max_v=2000)
-        koff = np.zeros(len(kv) + 1, dtype=np.uint64)
-        voff = np.zeros(len(kv) + 1, dtype=np.uint64)
-        np.cumsum([len(k) for k, _ in kv], out=koff[1:])
-        np.cumsum([len(v) for _, v in kv], out=voff[1:])
-        path = os.path.join(tmp, "ref%d.sst" % n)
-        err = C.create_string_buffer(256)
-        rc = lib.okv_write_sst(path.encode(), len(kv), b"".join(k for k, _ in kv) + b"\0", koff.ctypes.data,
-                               b"".join(v for _, v in kv) + b"\0", voff.ctypes.data, err, 256)
-        assert rc == 0, err.value
-        entries, props = sst.read_sst(open(path, "rb").read())
+        with open(os.path.join(G.GOLDEN, "ref_sst_%d.delta" % n), "rb") as f:
+            data = G.delta_decode(f.read(), gen_golden.sst_base(kv))
+        assert G.sha256(data) == want[str(n)], n
+        entries, props = sst.read_sst(data)
         assert [(k, t, v) for k, _, t, v in entries] == [(k, 1, v) for k, v in kv]
         assert props["external_version"] == 2 and props["global_seqno"] == 0 and props["num_entries"] == len(kv)
 
 
-def test_reference_ingests_files_written_here(ref_lib):
-    from oracle import okv
-    lib = _ref_extras(ref_lib)
-    tmp = tempfile.mkdtemp(dir="/dev/shm" if os.path.isdir("/dev/shm") else None)
-    for n, seed in ((1, 21), (200, 22), (5000, 23)):
+def test_reference_ingests_files_written_here():
+    """the files written here are byte for byte those the reference ingested when the fixtures were made, and what it
+    read back from them was this test's expectation"""
+    from oracle import gen_golden
+    want = G.load("reference_runs.json")["sst_ingest"]
+    for n, seed in gen_golden.SST_INGEST_CASES:
+        w = want[str(n)]
         kv = _kv(n, seed, max_v=1500)
-        path = os.path.join(tmp, "ours%d.sst" % n)
-        open(path, "wb").write(sst.write_sst(kv))
-        db = okv.Okv(lib)
-        err = C.create_string_buffer(256)
-        rc = lib.okv_ingest_sst(db.h, path.encode(), 1, err, 256)
-        assert rc == 0, err.value
-        assert db.latest_seq() == 0  # ingest into an empty DB does not consume sequence numbers
-        assert db.scan() == kv
-        for k, v in kv[:: max(1, len(kv) // 50)]:
-            assert db.get(k) == (0, v)
+        assert G.sha256(sst.write_sst(kv)) == w["file"], n
+        assert w["rc"] == 0
+        assert w["seq"] == 0  # ingest into an empty DB does not consume sequence numbers
+        assert w["scan"] == G.digest(kv)
+        assert w["gets"] == G.digest([(0, v) for _, v in kv[:: max(1, len(kv) // 50)]])
         # an overlapping second ingest is given global sequence number last+1 (rocksdb_assumption_test.cpp:272-283)
         kv2 = [(k, b"second:" + v[:5]) for k, v in kv[::3]]
-        path2 = os.path.join(tmp, "ours%d_b.sst" % n)
-        open(path2, "wb").write(sst.write_sst(kv2))
-        assert lib.okv_ingest_sst(db.h, path2.encode(), 1, err, 256) == 0, err.value
-        assert db.latest_seq() == 1
-        want = dict(kv)
-        want.update(kv2)
-        assert db.scan() == sorted(want.items())
+        data2 = sst.write_sst(kv2)
+        assert G.sha256(data2) == w["file2"], n
+        assert w["rc2"] == 0 and w["seq2"] == 1
+        want_kv = dict(kv)
+        want_kv.update(kv2)
+        assert w["scan2"] == G.digest(sorted(want_kv.items()))
         # (move_files = false: RocksDB stamps the sequence number into ITS copy; the file written here is untouched)
-        entries, props = sst.read_sst(open(path2, "rb").read())
+        assert w["file2_after"] == w["file2"]
+        entries, props = sst.read_sst(data2)
         assert props["global_seqno"] == 0 and [(k, v) for k, _, _, v in entries] == kv2
-        db.close()
 
 
 def test_shard_file_helpers_host_half():

@@ -1,9 +1,9 @@
-// randread_bench.cu — what can HBM3e on a B200 deliver for the MultiGet access pattern?
+// randread_bench.cu — what can HBM3 on an H100 deliver for the MultiGet access pattern?
 // Independent (no dependent chain) random reads: per lookup one 32-byte sector from an `idx_mb` MB index
 // region and one 96-byte entry (3 sectors, 32-byte aligned) from an `heap_mb` MB heap, 64 bytes written
 // out coalesced.  Addresses come from a hash of the thread id, so nothing is serialised: this is the
 // ceiling the dependent-chain kernel k_multi_get16 can approach with enough lookups in flight.
-//   nvcc -O3 -gencode arch=compute_100a,code=sm_100a -o randread_bench randread_bench.cu
+//   nvcc -O3 -gencode arch=compute_90a,code=sm_90a -o randread_bench randread_bench.cu
 #include <cstdio>
 #include <cstdint>
 #include <cstdlib>

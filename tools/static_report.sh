@@ -1,10 +1,10 @@
 #!/bin/bash
-# Static (no-GPU) evidence for profiles/: per-kernel registers / spills / shared memory from ptxas, and the SASS
+# Static (no-GPU) evidence: per-kernel registers / spills / shared memory from ptxas, and the SASS
 # mnemonics that show which hardware paths the kernels use (TMA bulk copy = UBLKCP, mbarrier = SYNCS, 128-bit
-# global loads, L2 cache-hint loads).  Usage: tools/static_report.sh > profiles/rNN_static_resources.txt
+# global loads, L2 cache-hint loads).  Usage: tools/static_report.sh > static_resources.txt
 set -e
 cd "$(dirname "$0")/../rocksplicator_b200/csrc"
-ARCH="-gencode arch=compute_100a,code=sm_100a"
+ARCH="-gencode arch=compute_90a,code=sm_90a"
 TMP=$(mktemp -d -p .)
 trap 'rm -rf "$TMP"' EXIT
 echo "# nvcc $ARCH -O3 -std=c++17 -lineinfo -Xptxas -v   ($(nvcc --version | grep release | sed 's/.*release //'))"

@@ -1,8 +1,9 @@
-"""Config-2 stretch point (SURVEY §8d): the largest per-shard count that fits — >= 100 GB of entries resident on one
-B200 — loaded through the apply path, compacted, then the same uniform MultiGet as bench.py (device-resident, CUDA
-events), every value of the last launch checked.  Shows whether the roofline fraction survives TLB / L2 pressure.
+"""Config-2 stretch point (SURVEY §8d): a per-shard count near what fits — 48 GB of entries (96 B a key) resident on one
+80 GB H100, beside the hash index, entry offsets and arena slack — loaded through the apply path,
+compacted, then the same uniform MultiGet as bench.py (device-resident, CUDA events), every value of the last launch
+checked.  Shows whether the roofline fraction survives TLB / L2 pressure.
 
-    python tools/stretch.py [--kv 1100000000] [--shards 1024] > profiles/r02_stretch.json
+    python tools/stretch.py [--kv 500000000] [--shards 1024] > stretch.json
 """
 import argparse, ctypes as C, json, os, sys, time
 import numpy as np
@@ -11,7 +12,7 @@ import torch
 from rocksplicator_b200 import engine, synth
 
 ap = argparse.ArgumentParser()
-ap.add_argument("--kv", type=int, default=1_000_000_000)
+ap.add_argument("--kv", type=int, default=500_000_000)
 ap.add_argument("--shards", type=int, default=1024)
 ap.add_argument("--steps", type=int, default=10)
 ap.add_argument("--warmup", type=int, default=3)
@@ -93,7 +94,7 @@ last = qs[W + K - 1]
 assert np.array_equal(d_vals.cpu().numpy().reshape(Q, 64), synth.values(seed, (last % np.uint64(S)).astype(np.int64), last, 0)), "parity"
 free, total = torch.cuda.mem_get_info()
 peak = json.load(open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "MEASURED_PEAKS.json")))["hbm_gbs"] if os.path.exists("MEASURED_PEAKS.json") else 6570.3
-print(json.dumps({"what": "config-2 stretch point: %d shards x %d KV (16 B / 64 B) resident on one B200, uniform MultiGet of %d lookups per launch, values of the last launch checked" % (S, NKV, Q),
+print(json.dumps({"what": "config-2 stretch point: %d shards x %d KV (16 B / 64 B) resident on one H100, uniform MultiGet of %d lookups per launch, values of the last launch checked" % (S, NKV, Q),
                   "run_bytes": run_bytes, "device_bytes_in_use": total - free, "load_s": t_load, "load_applies_per_s": NKV / t_load, "compact_s": t_compact,
                   "ms_per_launch": ms, "lookups_per_s": Q / ms * 1e3, "hbm_frac_of_peak_algorithmic": 168 * Q / (ms * 1e-3) / 1e9 / peak, "peak_gbs": peak}))
 eng.close()
