@@ -334,8 +334,11 @@ __device__ __forceinline__ void stg_pol(uint4* p, const uint4& v, u64 pol) {
 #ifndef RSP_MG_TPB
 #define RSP_MG_TPB 64
 #endif
+// 20 blocks of 64 threads per SM leave 48 registers per thread.  At 24 blocks (40 registers) ptxas for sm_90a spills
+// k_multi_get16<false> to local memory (60 bytes per thread), and the launch of 8.4 M lookups takes 1.04 ms instead of
+// 0.91 ms on an H100 80GB HBM3 at a 400 W power limit: the spill traffic costs more than the extra lookups in flight buy.
 #ifndef RSP_MG_MINB
-#define RSP_MG_MINB 24
+#define RSP_MG_MINB 20
 #endif
 
 // Candidate entry at `ent`: header unit 0, key unit KU, value units KU+1.. (U units in all).
