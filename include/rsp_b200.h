@@ -201,6 +201,36 @@ const uint8_t* rsp_iter_key(const rsp_iter* it, size_t* klen);
 const uint8_t* rsp_iter_value(const rsp_iter* it, size_t* vlen);
 int rsp_iter_status(const rsp_iter* it);
 
+/* ---- snapshots: DB::GetSnapshot / ReleaseSnapshot and reads with ReadOptions::snapshot ----------------------------
+ * A snapshot pins the shard's contents at creation: the memtable's contents are sorted into a private run, and that
+ * run and the shard's runs stay in HBM (even when merges replace them in the shard) until the snapshot and every
+ * iterator created at it are gone.  Reads at a snapshot run on the engine stream under the engine lock; they do not
+ * share launches with other readers.  Host-folded merge operators are finished on the host against the snapshot.
+ * rsp_snapshot_create answers RSP_BUSY while pre-staged ticks of the shard are in flight and when all
+ * RSP_MAX_SNAPSHOTS slots of the engine's snapshot table are taken.  rsp_shard_close answers RSP_BUSY while the shard
+ * has snapshots; rsp_engine_destroy releases the ones left.  While a snapshot is live, rsp_ingest_sorted gives the
+ * file a global sequence number (latest + 1) even when its range overlaps nothing, and refuses it with
+ * InvalidArgument unless allow_global_seqno (RocksDB's default snapshot_consistency = true). */
+#define RSP_MAX_SNAPSHOTS 4096
+typedef struct rsp_snapshot rsp_snapshot;
+int rsp_snapshot_create(rsp_shard* s, rsp_snapshot** out);
+void rsp_snapshot_release(rsp_snapshot* snap);
+uint64_t rsp_snapshot_seq(const rsp_snapshot* snap);  /* Snapshot::GetSequenceNumber: rsp_latest_seq at creation */
+uint32_t rsp_snapshot_slot(const rsp_snapshot* snap); /* the snapshot's index in the device form below */
+/* rsp_get at a snapshot */
+int rsp_get_at(const rsp_snapshot* snap, const uint8_t* key, size_t klen, uint8_t* val, size_t cap, size_t* vlen);
+/* rsp_multi_get with lookup i at snaps[i] (any shards of this engine); a NULL or foreign handle answers
+ * InvalidArgument for its lookup */
+int rsp_multi_get_at(rsp_engine* e, size_t n, rsp_snapshot* const* snaps, const uint8_t* keys, const uint64_t* koff,
+                     uint8_t* vals, size_t val_stride, uint32_t* vlen, int32_t* st);
+/* device form (as rsp_multi_get_device): lookup i reads at the snapshot whose slot is d_slot[i]; a slot that holds
+ * no snapshot answers InvalidArgument, a host-side merge operator 100.  The caller must not release a snapshot while
+ * its launches are in flight. */
+int rsp_multi_get_at_device(rsp_engine* e, size_t n, const uint32_t* d_slot, const uint8_t* d_keys, uint32_t klen,
+                            uint8_t* d_vals, uint32_t val_stride, uint32_t* d_vlen, int32_t* d_st, void* stream);
+/* an iterator over the snapshot: it holds its own pins and may outlive the snapshot */
+rsp_iter* rsp_iter_create_at(rsp_snapshot* snap);
+
 /* Batched range scans (BASELINE config 4: Seek + 128 x Next).  Memtables of the shards involved are flushed first
  * (the device form below scans the sorted runs only: call rsp_flush_all before it if memtables are not empty).  Scan i starts at the first key >=
  * start key i and returns up to max_entries live entries in key order.  Output i is a sequence of

@@ -179,6 +179,16 @@ struct rsp_shard {
   bool merging = false;           // a background merge of runs [bg_first_pinned ..] is in flight
   u64 uid = 0;                    // never reused: a background merge recognises the shard it planned for
   const Run* bg_first_pinned = nullptr;
+  u32 n_snapshots = 0;            // live rsp_snapshot handles on this shard
+};
+
+// DB::GetSnapshot: the shard's contents at one sequence number, as a pinned set of runs (the memtable's contents
+// sorted into a private run first).  Its ScanView sits in slot `slot` of the engine's snapshot table.
+struct rsp_snapshot {
+  rsp_shard* s;
+  u64 seq;
+  u32 slot;
+  std::vector<std::shared_ptr<Run>> pinned;
 };
 
 struct rsp_staged {
@@ -249,6 +259,9 @@ struct rsp_engine {
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   std::map<std::string, float> last_ms;
   std::atomic<u64> launches{0};
+  // snapshot table (allocated on the first snapshot): RSP_MAX_SNAPSHOTS views on the device, their owners on the host
+  ScanView* d_snap_views = nullptr;
+  std::vector<rsp_snapshot*> snap_slots;
 };
 
 static void set_err(rsp_shard* s, const std::string& m) {
@@ -685,6 +698,34 @@ static std::shared_ptr<Run> snapshot_memtable(rsp_engine* e, rsp_shard* s) {
   release_work(e, &plan);
   s->stats.compaction_bytes_read += (u64)s->h.mt_tail * 16;
   return plan.outs[0]->n_ent ? plan.outs[0] : nullptr;
+}
+
+static void view_of(const rsp_shard* s, const std::vector<std::shared_ptr<Run>>& pinned, ScanView* v) {
+  memset(v, 0, sizeof(*v));
+  v->n_runs = (u32)pinned.size();
+  v->merge_op = s->opts.merge_op;
+  for (u32 i = 0; i < v->n_runs; i++) v->runs[i] = pinned[i]->dev();
+}
+
+// The shard's current contents as a pinned, immutable set of runs, newest first: what an iterator or a snapshot
+// reads.  The memtable is unordered: its contents are sorted into a PRIVATE run (the same kernels as a flush), pinned
+// in front of the shard's runs.  The shard itself is not touched: no new run, no compaction trigger, writers go on
+// filling the same memtable (RocksDB: an iterator pins the memtable and the current version).  Merges may replace
+// the shard's runs later; the pinned ones stay in HBM until their last holder lets go.  Engine mutex held, no
+// pre-staged ticks in flight on the shard.
+static void pin_view(rsp_engine* e, rsp_shard* s, std::vector<std::shared_ptr<Run>>* pinned, ScanView* v) {
+  pinned->clear();
+  if (s->h.mt_count) {
+    wait_readers(e);
+    if (auto snap = snapshot_memtable(e, s)) pinned->push_back(snap);
+  }
+  pinned->insert(pinned->end(), s->runs.begin(), s->runs.end());
+  if (pinned->size() > RSP_MAX_RUNS) {  // the view has room for RSP_MAX_RUNS runs: fold the memtable in after all
+    pinned->clear();
+    compact_shards(e, {s}, false);
+    *pinned = s->runs;
+  }
+  view_of(s, *pinned, v);
 }
 
 // ---- background merges ------------------------------------------------------------------------------------
@@ -2081,6 +2122,8 @@ void rsp_engine_destroy(rsp_engine* e) {
   if (e->apply_comb) { e->apply_comb->destroy(); delete e->apply_comb; }
   cudaSetDevice(e->device);
   cudaStreamSynchronize(e->st);
+  for (rsp_snapshot* sn : e->snap_slots) delete sn;  // snapshots still held are released with their pins
+  if (e->d_snap_views) cudaFree(e->d_snap_views);
   for (rsp_shard* s : e->slots)
     if (s) { s->runs.clear(); delete s; }
   e->arena.destroy();
@@ -2156,7 +2199,7 @@ int rsp_shard_close(rsp_shard* s) {
   if (!s) return RSP_INVALID_ARGUMENT;
   rsp_engine* e = s->eng;
   std::lock_guard<std::mutex> g(e->mu);
-  if (ticks_in_flight(s)) return RSP_BUSY;
+  if (ticks_in_flight(s) || s->n_snapshots) return RSP_BUSY;  // (release the shard's snapshots first)
   CUDA_OK(cudaSetDevice(e->device));
   shard_close_locked(s);
   return RSP_OK;
@@ -2211,7 +2254,10 @@ int rsp_ingest_sorted(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_
     run_key_range(e, *r, &rf, &rl);
     if (!(hi < rf) && !(rl < lo)) { overlap = true; break; }
   }
-  if (overlap && !allow_global_seqno) {
+  // IngestExternalFileOptions::snapshot_consistency (default true): with a snapshot live the file takes a global
+  // sequence number even when it overlaps nothing, so that it is newer than every snapshot
+  const bool global_seqno = overlap || s->n_snapshots > 0;
+  if (global_seqno && !allow_global_seqno) {
     set_err(s, "Invalid argument: Global seqno is required, but disabled");
     return RSP_INVALID_ARGUMENT;
   }
@@ -2256,7 +2302,7 @@ int rsp_ingest_sorted(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_
       s->runs.insert(s->runs.begin(), tmp->runs[0]);
       tmp->runs.clear();
     }
-    if (overlap) {
+    if (global_seqno) {
       const u64 seq = s->last_seq.load() + 1;
       s->h.last_seq = seq;
       s->h.pub_seq = seq;
@@ -2706,28 +2752,30 @@ rsp_iter* rsp_iter_create(rsp_shard* s) {
   rsp_iter* it = new rsp_iter();
   it->s = s;
   CUDA_OK(cudaSetDevice(e->device));
-  // The memtable is unordered: its contents are sorted into a PRIVATE run (the same kernels as a flush), which the
-  // iterator pins in front of the shard's runs.  The shard itself is not touched: no new run, no compaction trigger,
-  // writers go on filling the same memtable (RocksDB: an iterator pins the memtable and the current version).
-  if (s->h.mt_count) {
-    wait_readers(e);
-    if (auto snap = snapshot_memtable(e, s)) it->pinned.push_back(snap);
-  }
-  it->pinned.insert(it->pinned.end(), s->runs.begin(), s->runs.end());
-  if (it->pinned.size() > RSP_MAX_RUNS) {  // the view has room for RSP_MAX_RUNS runs: fold the memtable in after all
-    it->pinned.clear();
-    compact_shards(e, {s}, false);
-    it->pinned = s->runs;
-  }
   ScanView v;
-  memset(&v, 0, sizeof(v));
-  v.n_runs = (u32)it->pinned.size();
-  v.merge_op = s->opts.merge_op;
-  for (u32 i = 0; i < v.n_runs; i++) v.runs[i] = it->pinned[i]->dev();
+  pin_view(e, s, &it->pinned, &v);
   it->d_view = (ScanView*)e->arena.alloc(sizeof(ScanView));
   CUDA_OK(cudaMemcpyAsync(it->d_view, &v, sizeof(v), cudaMemcpyHostToDevice, e->st));
   CUDA_OK(cudaStreamSynchronize(e->st));
   return it;
+  } catch (...) { abi_caught(); return nullptr; }
+}
+// an iterator over a snapshot's runs: it takes its own pins, so it may outlive the snapshot
+rsp_iter* rsp_iter_create_at(rsp_snapshot* snap) {
+  try {
+  if (!snap) return nullptr;
+  rsp_engine* e = snap->s->eng;
+  std::lock_guard<std::mutex> g(e->mu);
+  CUDA_OK(cudaSetDevice(e->device));
+  std::unique_ptr<rsp_iter> it(new rsp_iter());
+  it->s = snap->s;
+  it->pinned = snap->pinned;
+  ScanView v;
+  view_of(snap->s, it->pinned, &v);
+  it->d_view = (ScanView*)e->arena.alloc(sizeof(ScanView));
+  CUDA_OK(cudaMemcpyAsync(it->d_view, &v, sizeof(v), cudaMemcpyHostToDevice, e->st));
+  CUDA_OK(cudaStreamSynchronize(e->st));
+  return it.release();
   } catch (...) { abi_caught(); return nullptr; }
 }
 void rsp_iter_destroy(rsp_iter* it) {
@@ -2803,6 +2851,162 @@ const uint8_t* rsp_iter_value(const rsp_iter* it, size_t* vlen) {
   return (const uint8_t*)it->buf[it->pos].second.data();
 }
 int rsp_iter_status(const rsp_iter* it) { return it->status; }
+
+// ---- snapshots ----
+int rsp_snapshot_create(rsp_shard* s, rsp_snapshot** out) {
+  try {
+  if (!s || !out) return RSP_INVALID_ARGUMENT;
+  rsp_engine* e = s->eng;
+  std::lock_guard<std::mutex> g(e->mu);
+  if (ticks_in_flight(s)) return RSP_BUSY;  // fold the pre-staged ticks first (rsp_apply_staged_finish)
+  CUDA_OK(cudaSetDevice(e->device));
+  if (!e->d_snap_views) {
+    CUDA_OK(cudaMalloc(&e->d_snap_views, sizeof(ScanView) * RSP_MAX_SNAPSHOTS));
+    CUDA_OK(cudaMemset(e->d_snap_views, 0, sizeof(ScanView) * RSP_MAX_SNAPSHOTS));
+    e->snap_slots.assign(RSP_MAX_SNAPSHOTS, nullptr);
+  }
+  u32 slot = 0;
+  while (slot < RSP_MAX_SNAPSHOTS && e->snap_slots[slot]) slot++;
+  if (slot == RSP_MAX_SNAPSHOTS) return RSP_BUSY;
+  std::unique_ptr<rsp_snapshot> snap(new rsp_snapshot());
+  snap->s = s;
+  snap->slot = slot;
+  snap->seq = s->last_seq.load();
+  ScanView v;
+  pin_view(e, s, &snap->pinned, &v);
+  v.live = 1;
+  CUDA_OK(cudaMemcpyAsync(e->d_snap_views + slot, &v, sizeof(v), cudaMemcpyHostToDevice, e->st));
+  CUDA_OK(cudaStreamSynchronize(e->st));
+  e->snap_slots[slot] = snap.get();
+  s->n_snapshots++;
+  *out = snap.release();
+  return RSP_OK;
+  } catch (...) { return abi_caught(); }
+}
+
+void rsp_snapshot_release(rsp_snapshot* snap) {
+  try {
+  if (!snap) return;
+  rsp_engine* e = snap->s->eng;
+  std::lock_guard<std::mutex> g(e->mu);
+  CUDA_OK(cudaSetDevice(e->device));
+  wait_readers(e);  // (device-form reads on caller streams the engine knows of)
+  CUDA_OK(cudaMemsetAsync(e->d_snap_views + snap->slot, 0, sizeof(ScanView), e->st));
+  CUDA_OK(cudaStreamSynchronize(e->st));
+  e->snap_slots[snap->slot] = nullptr;
+  snap->s->n_snapshots--;
+  delete snap;  // runs that neither the shard nor another holder pins go back to the arena here
+  } catch (...) { abi_caught(); }
+}
+
+uint64_t rsp_snapshot_seq(const rsp_snapshot* snap) { return snap ? snap->seq : 0; }
+uint32_t rsp_snapshot_slot(const rsp_snapshot* snap) { return snap ? snap->slot : 0xffffffffu; }
+
+// MultiGet at snapshots over host buffers (engine mutex held): one launch of k_multi_get_at on the engine stream; the
+// rare statuses (host-folded merge operators, error texts) are finished on the host against the snapshot's view
+static int multi_get_at_locked(rsp_engine* e, size_t n, rsp_snapshot* const* snaps, const uint8_t* keys,
+                               const uint64_t* koff, uint8_t* vals, size_t val_stride, uint32_t* vlen, int32_t* st) {
+  if (n == 0) return RSP_OK;
+  std::vector<u32> slot(n);
+  for (size_t i = 0; i < n; i++) slot[i] = snaps[i] && snaps[i]->s->eng == e ? snaps[i]->slot : 0xffffffffu;
+  const size_t key_bytes = (size_t)koff[n];
+  const size_t o_koff = align_up(n * 4, 256), o_keys = o_koff + align_up((n + 1) * 8, 256);
+  const size_t o_vlen = o_keys + align_up(key_bytes + 16, 256), o_st = o_vlen + align_up(n * 4, 256);
+  const size_t o_spec = o_st + align_up(n * 4, 256), o_vals = o_spec + 256;
+  u8* d = (u8*)e->dev_q.get(o_vals + n * val_stride + 256);
+  CUDA_OK(cudaMemcpyAsync(d, slot.data(), n * 4, cudaMemcpyHostToDevice, e->st));
+  CUDA_OK(cudaMemcpyAsync(d + o_koff, koff, (n + 1) * 8, cudaMemcpyHostToDevice, e->st));
+  if (key_bytes) CUDA_OK(cudaMemcpyAsync(d + o_keys, keys, key_bytes, cudaMemcpyHostToDevice, e->st));
+  CUDA_OK(cudaMemsetAsync(d + o_spec, 0, 4, e->st));
+  GetAtArgs a;
+  a.views = e->d_snap_views; a.slot = (const u32*)d; a.keys = d + o_keys; a.koff = (const u64*)(d + o_koff);
+  a.vals = d + o_vals; a.val_stride = val_stride; a.vlen = (u32*)(d + o_vlen); a.st = (i32*)(d + o_st);
+  a.n_special = (u32*)(d + o_spec); a.n_views = e->d_snap_views ? RSP_MAX_SNAPSHOTS : 0; a.klen_fixed = 0; a.n = (u32)n;
+  CUDA_OK(cudaEventRecord(e->ev0, e->st));
+  launch_multi_get_at(a, e->st);
+  CUDA_OK(cudaGetLastError());
+  e->launches++;
+  CUDA_OK(cudaEventRecord(e->ev1, e->st));
+  u32 n_special = 0;
+  CUDA_OK(cudaMemcpyAsync(vlen, d + o_vlen, n * 4, cudaMemcpyDeviceToHost, e->st));
+  CUDA_OK(cudaMemcpyAsync(st, d + o_st, n * 4, cudaMemcpyDeviceToHost, e->st));
+  if (val_stride) CUDA_OK(cudaMemcpyAsync(vals, d + o_vals, n * val_stride, cudaMemcpyDeviceToHost, e->st));
+  CUDA_OK(cudaMemcpyAsync(&n_special, d + o_spec, 4, cudaMemcpyDeviceToHost, e->st));
+  CUDA_OK(cudaStreamSynchronize(e->st));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
+  e->last_ms["multi_get_at"] = ms;
+  if (!n_special) return RSP_OK;
+  for (size_t i = 0; i < n; i++) {
+    if (slot[i] == 0xffffffffu) continue;  // InvalidArgument, no text
+    rsp_shard* s = snaps[i]->s;
+    if (st[i] == ST_NEED_HOST_MERGE) {
+      std::string v;
+      const int rc = host_fold_get(e, s, keys + koff[i], (size_t)(koff[i + 1] - koff[i]), &v, e->d_snap_views + slot[i]);
+      st[i] = rc;
+      vlen[i] = 0;
+      if (rc == RSP_OK) {
+        vlen[i] = (u32)v.size();
+        if (v.size() > val_stride) st[i] = RSP_INCOMPLETE;
+        else memcpy(vals + i * val_stride, v.data(), v.size());
+      }
+    } else if (!plain_status(st[i])) {
+      const u32 msg = vlen[i];
+      set_err(s, msg < MSG_COUNT ? kMsgText[msg] : "error");
+      vlen[i] = 0;
+    }
+  }
+  return RSP_OK;
+}
+
+int rsp_get_at(const rsp_snapshot* snap, const uint8_t* key, size_t klen, uint8_t* val, size_t cap, size_t* vlen) {
+  try {
+  if (!snap) return RSP_INVALID_ARGUMENT;
+  rsp_engine* e = snap->s->eng;
+  rsp_snapshot* sp = const_cast<rsp_snapshot*>(snap);
+  const uint64_t koff[2] = {0, klen};
+  static const uint8_t empty = 0;
+  uint32_t vl = 0;
+  int32_t st = 0;
+  std::lock_guard<std::mutex> g(e->mu);
+  CUDA_OK(cudaSetDevice(e->device));
+  const int rc = multi_get_at_locked(e, 1, &sp, key ? key : &empty, koff, val, val ? cap : 0, &vl, &st);
+  if (rc != RSP_OK) return rc;
+  if (vlen) *vlen = vl;
+  return st;
+  } catch (...) { return abi_caught(); }
+}
+
+int rsp_multi_get_at(rsp_engine* e, size_t n, rsp_snapshot* const* snaps, const uint8_t* keys, const uint64_t* koff,
+                     uint8_t* vals, size_t val_stride, uint32_t* vlen, int32_t* st) {
+  try {
+  if (!e || (n && (!snaps || !koff || !vlen || !st || (val_stride && !vals)))) return RSP_INVALID_ARGUMENT;
+  std::lock_guard<std::mutex> g(e->mu);
+  CUDA_OK(cudaSetDevice(e->device));
+  return multi_get_at_locked(e, n, snaps, keys, koff, vals, val_stride, vlen, st);
+  } catch (...) { return abi_caught(); }
+}
+
+int rsp_multi_get_at_device(rsp_engine* e, size_t n, const uint32_t* d_slot, const uint8_t* d_keys, uint32_t klen,
+                            uint8_t* d_vals, uint32_t val_stride, uint32_t* d_vlen, int32_t* d_st, void* stream) {
+  try {
+  if (!e || !klen) return RSP_INVALID_ARGUMENT;
+  GetAtArgs a;
+  a.slot = d_slot; a.keys = d_keys; a.koff = nullptr; a.klen_fixed = klen; a.vals = d_vals; a.val_stride = val_stride;
+  a.vlen = d_vlen; a.st = d_st; a.n_special = nullptr; a.n = (u32)n;
+  {
+    std::lock_guard<std::mutex> g(e->mu);
+    cudaStream_t rs = stream ? (cudaStream_t)stream : e->st;
+    a.views = e->d_snap_views;
+    a.n_views = e->d_snap_views ? RSP_MAX_SNAPSHOTS : 0;
+    reader_begin(e, rs);
+    launch_multi_get_at(a, rs);
+    reader_end(e, rs);
+  }
+  e->launches++;
+  return cudaPeekAtLastError() == cudaSuccess ? RSP_OK : RSP_IO_ERROR;
+  } catch (...) { return abi_caught(); }
+}
 
 // ---- batched scans (host buffers) ----
 int rsp_multi_scan(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,

@@ -795,6 +795,74 @@ void launch_get_versions(const VersionsArgs& a, cudaStream_t s) {
 }
 
 // ------------------------------------------------------------------------------------------------
+// k_multi_get_at — MultiGet at snapshots: the generic eight-lane walk over a pinned view instead of a live shard
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256) k_multi_get_at(GetAtArgs a) {
+  const u32 q = (blockIdx.x * blockDim.x + threadIdx.x) / MG_LANES;
+  const u32 lane = threadIdx.x & (MG_LANES - 1);
+  const u32 gbase = (threadIdx.x & 31u) & ~(MG_LANES - 1u);
+  const u32 gmask = ((1u << MG_LANES) - 1u) << gbase;
+  if (q >= a.n) return;
+  const u32 slot = __ldg(a.slot + q);
+  if (slot >= a.n_views || !a.views[slot].live) {  // null, released or foreign snapshot
+    if (lane == 0) {
+      a.st[q] = 4;
+      a.vlen[q] = 0;
+      if (a.n_special) atomicAdd(a.n_special, 1u);
+    }
+    return;
+  }
+  const ScanView& vw = a.views[slot];
+  const u8* kp;
+  u32 klen;
+  if (a.klen_fixed) {
+    klen = a.klen_fixed;
+    kp = a.keys + (u64)q * klen;
+  } else {
+    const u64 o = __ldg(a.koff + q);
+    klen = (u32)(__ldg(a.koff + q + 1) - o);
+    kp = a.keys + o;
+  }
+  Acc acc;
+  acc.init(vw.merge_op);
+  const u64 h = hash_key(kp, klen);
+  const u32 n_runs = vw.n_runs;
+  for (u32 ri = 0; ri < n_runs && !acc.done; ri++) walk_run<MG_LANES>(vw.runs[ri], kp, klen, h, lane, gmask, gbase, acc);
+  acc.end_of_versions();
+  i32 st = acc.status;
+  u32 vlen = 0;
+  if (st == 0) {
+    vlen = acc.res_len;
+    if ((u64)vlen > a.val_stride) {
+      st = 7;  // RSP_INCOMPLETE: vlen reports the size needed
+    } else {
+      u8* dst = a.vals + (u64)q * a.val_stride;
+      if (acc.imm) {
+        if (lane == 0) {
+#pragma unroll
+          for (u32 b = 0; b < 8; b++) dst[b] = (u8)(acc.res_imm >> (8u * b));
+        }
+      } else {
+        group_copy_out(dst, acc.res_ptr, vlen, lane, MG_LANES);
+      }
+    }
+  } else if (st != 1 && st != ST_NEED_HOST_MERGE) {
+    vlen = acc.msg;  // message id rides in vlen for error statuses
+  }
+  if (lane == 0) {
+    a.st[q] = st;
+    a.vlen[q] = vlen;
+    if (st != 0 && st != 1 && st != 7 && a.n_special) atomicAdd(a.n_special, 1u);
+  }
+}
+
+void launch_multi_get_at(const GetAtArgs& a, cudaStream_t s) {
+  if (!a.n) return;
+  const u32 per_block = 256 / MG_LANES;
+  k_multi_get_at<<<(a.n + per_block - 1) / per_block, 256, 0, s>>>(a);
+}
+
+// ------------------------------------------------------------------------------------------------
 // k_multi_scan — Seek + N x Next/Prev over the sorted runs (one warp per scan)
 // ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ int cmp_run_key(const RunDev& r, u32 ord, const u8* kp, u32 klen) {

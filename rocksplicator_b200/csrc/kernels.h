@@ -168,8 +168,27 @@ struct ScanView {
   RunDev runs[RSP_MAX_RUNS];
   u32 n_runs;
   u32 merge_op;
-  u32 pad0, pad1;
+  u32 live;  // snapshot table slots: 1 while the snapshot is held (k_multi_get_at answers InvalidArgument otherwise)
+  u32 pad1;
 };
+
+// point lookups at snapshots: lookup q walks the pinned view views[slot[q]] (sorted runs only, newest first) with
+// eight lanes, and answers like k_multi_get (status 100 = a host-side merge operator must finish it)
+struct GetAtArgs {
+  const ScanView* views;  // the engine's snapshot table
+  const u32* slot;        // [n]
+  const u8* keys;
+  const u64* koff;        // [n+1] or nullptr when klen_fixed > 0
+  u8* vals;               // value i at vals + i * val_stride
+  u64 val_stride;
+  u32* vlen;              // [n]
+  i32* st;                // [n]
+  u32* n_special;         // [1] counts statuses other than OK / NotFound / Incomplete (may be nullptr)
+  u32 n_views;            // table capacity (0 = no table yet): slots >= this answer InvalidArgument
+  u32 klen_fixed;
+  u32 n;
+};
+void launch_multi_get_at(const GetAtArgs& a, cudaStream_t s);
 // vlen markers in scan records (the value is absent: the record is [u32 klen][u32 marker][key])
 constexpr u32 SCAN_VLEN_HOST_FOLD = 0xffffffffu;     // the merge operator lives on the host: fold this key there
 constexpr u32 SCAN_VLEN_MERGE_FAILED = 0xfffffffeu;  // the merge failed: empty value, the scan's st holds the status

@@ -83,6 +83,16 @@ EXPORTS = {
     "rsp_iter_key": (C.c_void_p, [C.c_void_p, C.POINTER(C.c_size_t)]),
     "rsp_iter_value": (C.c_void_p, [C.c_void_p, C.POINTER(C.c_size_t)]),
     "rsp_iter_status": (C.c_int, [C.c_void_p]),
+    "rsp_snapshot_create": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
+    "rsp_snapshot_release": (None, [C.c_void_p]),
+    "rsp_snapshot_seq": (C.c_uint64, [C.c_void_p]),
+    "rsp_snapshot_slot": (C.c_uint32, [C.c_void_p]),
+    "rsp_get_at": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t, C.c_void_p, C.c_size_t, C.POINTER(C.c_size_t)]),
+    "rsp_multi_get_at": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_size_t, C.c_void_p, C.c_void_p]),
+    "rsp_multi_get_at_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
+                                          C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rsp_iter_create_at": (C.c_void_p, [C.c_void_p]),
     "rsp_multi_scan": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
                                  C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     "rsp_flush": (C.c_int, [C.c_void_p]),
@@ -135,9 +145,9 @@ def _ptr(a):
 
 
 class Iterator:
-    def __init__(self, shard):
+    def __init__(self, shard, snapshot=None):
         self.lib = shard.lib
-        self.h = self.lib.rsp_iter_create(shard.h)
+        self.h = self.lib.rsp_iter_create(shard.h) if snapshot is None else self.lib.rsp_iter_create_at(snapshot.h)
         self._shard = shard
 
     def close(self):
@@ -168,6 +178,62 @@ class Iterator:
         n = C.c_size_t()
         p = self.lib.rsp_iter_value(self.h, C.byref(n))
         return C.string_at(p, n.value) if n.value else b""
+
+
+class Snapshot:
+    """DB::GetSnapshot on one shard: reads through it see the shard as it was at `seq`.  Release it (or leave the
+    `with` block) to let go of the HBM it pins; iterators created from it keep their own pins."""
+
+    def __init__(self, shard):
+        self.shard = shard
+        self.lib = shard.lib
+        h = C.c_void_p()
+        rc = self.lib.rsp_snapshot_create(shard.h, C.byref(h))
+        if rc != OK:
+            raise RuntimeError(f"rsp_snapshot_create({shard.name}) -> {rc}")
+        self.h = h
+        self.seq = self.lib.rsp_snapshot_seq(h)
+        self.slot = self.lib.rsp_snapshot_slot(h)
+
+    def release(self):
+        if self.h:
+            self.lib.rsp_snapshot_release(self.h)
+            self.h = None
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, *exc):
+        self.release()
+
+    def get(self, key: bytes, cap: int = 256):
+        while True:
+            buf = C.create_string_buffer(max(cap, 1))
+            n = C.c_size_t()
+            rc = self.lib.rsp_get_at(self.h, key, len(key), buf, cap, C.byref(n))
+            if rc == INCOMPLETE:
+                cap = n.value
+                continue
+            return (rc, buf.raw[:n.value]) if rc == OK else (rc, None)
+
+    def multi_get(self, keys, stride=256):
+        return self.shard.engine.multi_get_at([self] * len(keys), keys, stride)
+
+    def iterator(self):
+        return Iterator(self.shard, self)
+
+    def scan(self, start=None, limit=None):
+        it = self.iterator()
+        if start is None:
+            it.seek_to_first()
+        else:
+            it.seek(start)
+        out = []
+        while it.valid() and (limit is None or len(out) < limit):
+            out.append((it.key(), it.value()))
+            it.next()
+        it.close()
+        return out
 
 
 class Shard:
@@ -227,6 +293,9 @@ class Shard:
 
     def iterator(self):
         return Iterator(self)
+
+    def snapshot(self):
+        return Snapshot(self)
 
     def scan(self, start=None, limit=None):
         it = self.iterator()
@@ -331,6 +400,27 @@ class Engine:
             for i in range(n):
                 out.append((int(st[i]), vals[i * stride:i * stride + vlen[i]].tobytes() if st[i] == OK else None))
             return out
+
+    def multi_get_at(self, snapshots, keys, stride=256):
+        """lookup i at snapshots[i] (a Snapshot, or None: InvalidArgument) -> [(status, value|None)]"""
+        n = len(keys)
+        handles = (C.c_void_p * max(n, 1))(*[s.h if s is not None else None for s in snapshots])
+        off = np.zeros(n + 1, dtype=np.uint64)
+        np.cumsum(np.fromiter((len(k) for k in keys), dtype=np.uint64, count=n), out=off[1:])
+        blob = np.frombuffer(b"".join(keys) + b"\0", dtype=np.uint8)
+        while True:
+            vals = np.zeros(max(n * stride, 1), dtype=np.uint8)
+            vlen = np.zeros(max(n, 1), dtype=np.uint32)
+            st = np.zeros(max(n, 1), dtype=np.int32)
+            rc = self.lib.rsp_multi_get_at(self.h, n, handles, _ptr(blob), _ptr(off), _ptr(vals), stride,
+                                           _ptr(vlen), _ptr(st))
+            if rc != OK:
+                raise RuntimeError(f"rsp_multi_get_at -> {rc}")
+            if n and (st[:n] == INCOMPLETE).any():
+                stride = int(vlen[:n][st[:n] == INCOMPLETE].max())
+                continue
+            return [(int(st[i]), vals[i * stride:i * stride + vlen[i]].tobytes() if st[i] == OK else None)
+                    for i in range(n)]
 
     def multi_get_fixed(self, six, keys, klen, vals, stride, vlen, st):
         """numpy arrays in place (pinned or pageable host memory)."""

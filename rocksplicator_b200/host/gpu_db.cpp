@@ -154,8 +154,39 @@ bool ReadWholeFile(const std::string& path, std::string* out) {
 }
 }  // namespace
 
+namespace {
+class GpuSnapshot : public rocksdb::Snapshot {
+ public:
+  explicit GpuSnapshot(rsp_snapshot* s) : s_(s) {}
+  ~GpuSnapshot() override {}
+  rocksdb::SequenceNumber GetSequenceNumber() const override { return rsp_snapshot_seq(s_); }
+  rsp_snapshot* raw() const { return s_; }
+
+ private:
+  rsp_snapshot* s_;
+};
+rsp_snapshot* RawSnapshot(const rocksdb::Snapshot* s) { return static_cast<const GpuSnapshot*>(s)->raw(); }
+}  // namespace
+
+const rocksdb::Snapshot* GpuDB::GetSnapshot() {
+  rsp_snapshot* s = nullptr;
+  if (rsp_snapshot_create(shard_, &s) != RSP_OK) return nullptr;
+  n_snapshots_++;
+  return new GpuSnapshot(s);
+}
+
+void GpuDB::ReleaseSnapshot(const rocksdb::Snapshot* snapshot) {
+  if (!snapshot) return;
+  rsp_snapshot_release(RawSnapshot(snapshot));
+  n_snapshots_--;
+  delete static_cast<const GpuSnapshot*>(snapshot);
+}
+
 Status GpuDB::IngestExternalFile(const std::vector<std::string>& files, const rocksdb::IngestExternalFileOptions& opt) {
   if (files.empty()) return Status::InvalidArgument("external_files is empty");
+  // the engine cannot show a file to snapshots taken before it: with snapshots live, the file is always newer
+  if (!opt.snapshot_consistency && n_snapshots_.load() > 0)
+    return Status::NotSupported("IngestExternalFile without snapshot_consistency while snapshots are live");
   struct Parsed { std::vector<sst::Entry> entries; };
   std::vector<Parsed> parsed(files.size());
   for (size_t i = 0; i < files.size(); i++) {
@@ -404,11 +435,12 @@ void GpuDB::ApplyReplicatedBatch(const std::vector<replicator::Update>& updates,
   }
 }
 
-Status GpuDB::Get(const rocksdb::ReadOptions&, const Slice& key, std::string* value) {
+Status GpuDB::Get(const rocksdb::ReadOptions& o, const Slice& key, std::string* value) {
   size_t cap = 256, n = 0;
   for (;;) {
     value->resize(cap);
-    const int rc = rsp_get(shard_, (const uint8_t*)key.data(), key.size(), (uint8_t*)&(*value)[0], cap, &n);
+    const int rc = o.snapshot ? rsp_get_at(RawSnapshot(o.snapshot), (const uint8_t*)key.data(), key.size(), (uint8_t*)&(*value)[0], cap, &n)
+                              : rsp_get(shard_, (const uint8_t*)key.data(), key.size(), (uint8_t*)&(*value)[0], cap, &n);
     if (rc == RSP_INCOMPLETE) { cap = n; continue; }
     if (rc != RSP_OK) { value->clear(); return rc == RSP_NOT_FOUND ? Status::NotFound() : ToStatus(rc); }
     value->resize(n);
@@ -422,7 +454,43 @@ Status GpuDB::Get(const rocksdb::ReadOptions& o, rocksdb::ColumnFamilyHandle*, c
   return s;
 }
 
-std::vector<Status> GpuDB::MultiGet(const rocksdb::ReadOptions&, const std::vector<Slice>& keys, std::vector<std::string>* values) {
+// MultiGet at a snapshot (rsp_multi_get_at): values larger than the stride come back Incomplete with their size, and
+// the call is repeated with a stride that fits them
+std::vector<Status> GpuDB::MultiGetAt(const rocksdb::Snapshot* snapshot, const std::vector<Slice>& keys,
+                                      std::vector<std::string>* values) {
+  const size_t n = keys.size();
+  std::vector<Status> out(n);
+  values->assign(n, std::string());
+  if (!n) return out;
+  std::string blob;
+  std::vector<uint64_t> koff(n + 1, 0);
+  for (size_t i = 0; i < n; i++) { blob.append(keys[i].data(), keys[i].size()); koff[i + 1] = blob.size(); }
+  blob.push_back('\0');
+  std::vector<rsp_snapshot*> snaps(n, RawSnapshot(snapshot));
+  std::vector<uint32_t> vlen(n);
+  std::vector<int32_t> st(n);
+  size_t stride = std::max<size_t>(256, value_hint_.load(std::memory_order_relaxed));
+  for (;;) {
+    std::vector<uint8_t> vals(n * stride);
+    const int rc = rsp_multi_get_at(engine(), n, snaps.data(), (const uint8_t*)blob.data(), koff.data(), vals.data(), stride,
+                                    vlen.data(), st.data());
+    if (rc != RSP_OK) {
+      for (auto& s : out) s = Status::IOError("rsp_multi_get_at");
+      return out;
+    }
+    size_t more = 0;
+    for (size_t i = 0; i < n; i++) if (st[i] == RSP_INCOMPLETE) more = std::max<size_t>(more, vlen[i]);
+    if (more) { stride = more; continue; }
+    for (size_t i = 0; i < n; i++) {
+      if (st[i] == RSP_OK) (*values)[i].assign((const char*)&vals[i * stride], vlen[i]);
+      else out[i] = st[i] == RSP_NOT_FOUND ? Status::NotFound() : ToStatus(st[i]);
+    }
+    return out;
+  }
+}
+
+std::vector<Status> GpuDB::MultiGet(const rocksdb::ReadOptions& options, const std::vector<Slice>& keys, std::vector<std::string>* values) {
+  if (options.snapshot) return MultiGetAt(options.snapshot, keys, values);
   const size_t n = keys.size();
   std::vector<Status> out(n);
   values->assign(n, std::string());
@@ -474,7 +542,9 @@ class GpuIterator : public rocksdb::Iterator {
 };
 }  // namespace
 
-rocksdb::Iterator* GpuDB::NewIterator(const rocksdb::ReadOptions&) { return new GpuIterator(rsp_iter_create(shard_)); }
+rocksdb::Iterator* GpuDB::NewIterator(const rocksdb::ReadOptions& o) {
+  return new GpuIterator(o.snapshot ? rsp_iter_create_at(RawSnapshot(o.snapshot)) : rsp_iter_create(shard_));
+}
 
 Status GpuDB::CompactRange(const rocksdb::CompactRangeOptions&, const Slice* begin, const Slice* end) {
   if (begin || end) return Status::NotSupported("partial CompactRange");  // the reference passes (nullptr, nullptr)

@@ -68,6 +68,9 @@ class GpuDB : public rocksdb::DB {
   static rocksdb::Status Restore(const rocksdb::Options& options, const std::string& name, const std::string& dir,
                                  rocksdb::DB** dbptr, int device = 0);
   rocksdb::SequenceNumber GetLatestSequenceNumber() const override;
+  // rsp_snapshot_create / rsp_snapshot_release; nullptr when the engine cannot take one (its snapshot table is full)
+  const rocksdb::Snapshot* GetSnapshot() override;
+  void ReleaseSnapshot(const rocksdb::Snapshot* snapshot) override;
   rocksdb::Status GetUpdatesSince(rocksdb::SequenceNumber seq,
                                   std::unique_ptr<rocksdb::TransactionLogIterator>* iter) override;
   rocksdb::ColumnFamilyHandle* DefaultColumnFamily() const override { return &default_cf_; }
@@ -122,7 +125,10 @@ class GpuDB : public rocksdb::DB {
   void LogPush(std::shared_ptr<const LogChunk> c);  // log_mu_ held
   size_t log_bytes_ = 0;
   size_t log_cap_bytes_ = 256u << 20;
-  std::atomic<size_t> value_hint_{0};  // largest value MultiGet has seen (the staging stride of its first pass)
+  std::atomic<size_t> value_hint_{0};
+  std::atomic<int> n_snapshots_{0};  // live GetSnapshot handles
+  std::vector<rocksdb::Status> MultiGetAt(const rocksdb::Snapshot* snapshot, const std::vector<rocksdb::Slice>& keys,
+                                          std::vector<std::string>* values);  // largest value MultiGet has seen (the staging stride of its first pass)
 };
 
 // Spills shards on a schedule: every `period_ms` each registered DB whose sequence number moved since its last backup

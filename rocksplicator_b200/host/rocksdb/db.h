@@ -17,6 +17,15 @@
 
 namespace rocksdb {
 
+// DB::GetSnapshot's handle: the DB as of GetSequenceNumber(); released with DB::ReleaseSnapshot
+class Snapshot {
+ public:
+  virtual SequenceNumber GetSequenceNumber() const = 0;
+
+ protected:
+  virtual ~Snapshot() {}
+};
+
 class ColumnFamilyHandle {
  public:
   virtual ~ColumnFamilyHandle() {}
@@ -43,6 +52,8 @@ class DB {
     return Status::NotSupported("IngestExternalFile");
   }
   virtual SequenceNumber GetLatestSequenceNumber() const = 0;
+  virtual const Snapshot* GetSnapshot() { return nullptr; }
+  virtual void ReleaseSnapshot(const Snapshot* /*snapshot*/) {}
   virtual Status GetUpdatesSince(SequenceNumber seq, std::unique_ptr<TransactionLogIterator>* iter) = 0;
   virtual ColumnFamilyHandle* DefaultColumnFamily() const = 0;
   virtual Options GetOptions() const = 0;
