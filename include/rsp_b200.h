@@ -263,7 +263,11 @@ int rsp_ingest_sorted(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_
  * `stream` is a cudaStream_t passed as void* (0 = the engine's own read stream).  No host
  * synchronisation is performed; the caller owns ordering and timing.  A lookup that needs a host-side merge operator
  * (RSP_MERGE_CALLBACK shards with merge operands on the key) cannot be finished on the device: its d_st is 100 and the
- * caller resolves it with rsp_get / rsp_multi_get. */
+ * caller resolves it with rsp_get / rsp_multi_get.  rsp_multi_scan_device scans the sorted runs only: on a shard whose
+ * memtable holds writes it returns the runs' contents with d_st = 0, without those writes.  Flush such shards first, or
+ * use rsp_multi_scan, which does.
+ * Reads on a caller's stream are ordered against the engine's own work: they wait for a flush, compaction or close issued
+ * before them, and such a call issued after them waits for them before it returns. */
 int rsp_multi_get_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys,
                          uint32_t klen, uint8_t* d_vals, uint32_t val_stride, uint32_t* d_vlen,
                          int32_t* d_st, void* stream);

@@ -13,7 +13,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "librsp_b200.so")
 SOURCES = ["k_apply.cu", "k_read.cu", "k_compact.cu", "engine.cu"]
-HEADERS = ["format.cuh", "kernels.h", "stager.h", "arena.h", os.path.join("..", "..", "include", "rsp_b200.h")]
+HEADERS = ["format.cuh", "kernels.h", "stager.h", "arena.h", "reader_set.h", os.path.join("..", "..", "include", "rsp_b200.h")]
 NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC", "-Xcompiler", "-Wall"] + os.environ.get("RSP_NVCC_EXTRA", "").split()
 

@@ -25,6 +25,7 @@
 
 #include "../../include/rsp_b200.h"
 #include "arena.h"
+#include "reader_set.h"
 #include "stager.h"
 #include "kernels.h"
 
@@ -213,6 +214,19 @@ struct ReadCombiner;
 struct ApplyCombiner;
 struct Compactor;
 
+struct CudaReaderApi {  // ReaderSet's stream / event operations
+  using Stream = cudaStream_t;
+  using Event = cudaEvent_t;
+  static Event create() {
+    cudaEvent_t ev = nullptr;
+    CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    return ev;
+  }
+  static void record(Event ev, Stream s) { CUDA_OK(cudaEventRecord(ev, s)); }
+  static void wait(Stream on, Event ev) { CUDA_OK(cudaStreamWaitEvent(on, ev, 0)); }
+  static void destroy(Event ev) { cudaEventDestroy(ev); }
+};
+
 struct rsp_engine {
   int device = 0;
   // staging combiners (created on first use): concurrent readers / writers share device batches (stager.h)
@@ -241,8 +255,7 @@ struct rsp_engine {
   std::vector<u32> gid_scratch;
   std::vector<u8> seen_scratch;
   // ordering between reads launched on caller streams and memtable flushes / re-allocations on the engine stream
-  cudaEvent_t reader_ev[8] = {};
-  u32 reader_head = 0, reader_pending = 0;
+  ReaderSet<CudaReaderApi> readers;
   cudaEvent_t mut_ev = nullptr;
   bool mut_recorded = false;
   size_t stage_threads = 1;
@@ -269,14 +282,11 @@ static void set_err(rsp_shard* s, const std::string& m) {
   s->last_error = m;
 }
 
-// Reads launched on a caller's stream (rsp_multi_get_device / rsp_multi_scan_device) are lock-free against apply
-// ticks, but a flush or a memtable re-allocation recycles memory they may be reading: the engine stream waits for
-// the outstanding reader events first, and later reads wait for the mutation event.
-static void wait_readers(rsp_engine* e) {
-  const u32 n = std::min<u32>(e->reader_pending, 8);
-  for (u32 k = 0; k < n; k++) CUDA_OK(cudaStreamWaitEvent(e->st, e->reader_ev[(e->reader_head + 8 - 1 - k) % 8], 0));
-  e->reader_pending = 0;
-}
+// Reads launched on a stream other than the engine's (the device forms on a caller's stream, the read combiner on its
+// own) are lock-free against apply ticks, but a flush, a memtable re-allocation, a merge install, a snapshot's
+// memtable pin or a shard close recycles or clears memory they may be reading: the engine stream first waits for the
+// latest read on every such stream (reader_set.h), and later reads wait for the mutation event.
+static void wait_readers(rsp_engine* e) { e->readers.wait(e->st); }
 static void note_mutation(rsp_engine* e) {
   CUDA_OK(cudaEventRecord(e->mut_ev, e->st));
   e->mut_recorded = true;
@@ -286,9 +296,7 @@ static void reader_begin(rsp_engine* e, cudaStream_t s) {
 }
 static void reader_end(rsp_engine* e, cudaStream_t s) {
   if (s == e->st) return;
-  CUDA_OK(cudaEventRecord(e->reader_ev[e->reader_head], s));
-  e->reader_head = (e->reader_head + 1) % 8;
-  e->reader_pending++;
+  e->readers.note(s);
 }
 
 // runs_only: only the run set changed (a background merge was installed).  The sequencing state of the descriptor
@@ -2069,7 +2077,6 @@ int rsp_engine_create(int device, const rsp_engine_cfg* cfg, rsp_engine** out) {
     CUDA_OK(cudaStreamCreateWithFlags(&e->cs[k], cudaStreamNonBlocking));
     CUDA_OK(cudaEventCreateWithFlags(&e->cs_done[k], cudaEventDisableTiming));
   }
-  for (int k = 0; k < 8; k++) CUDA_OK(cudaEventCreateWithFlags(&e->reader_ev[k], cudaEventDisableTiming));
   CUDA_OK(cudaEventCreateWithFlags(&e->mut_ev, cudaEventDisableTiming));
   CUDA_OK(cudaEventCreate(&e->ev0));
   CUDA_OK(cudaEventCreate(&e->ev1));
@@ -2131,7 +2138,7 @@ void rsp_engine_destroy(rsp_engine* e) {
   cudaFree(e->d_shards);
   cudaFree(e->d_fast);
   cudaEventDestroy(e->ev0); cudaEventDestroy(e->ev1); cudaEventDestroy(e->up_ev); cudaEventDestroy(e->pending_ev);
-  for (int k = 0; k < 8; k++) cudaEventDestroy(e->reader_ev[k]);
+  e->readers.destroy();
   cudaEventDestroy(e->mut_ev);
   for (int k = 0; k < 3; k++) { cudaStreamDestroy(e->cs[k]); cudaEventDestroy(e->cs_done[k]); }
   cudaStreamDestroy(e->st);
