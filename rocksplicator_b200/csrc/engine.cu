@@ -246,7 +246,7 @@ struct rsp_engine {
   std::vector<rsp_shard*> slots;
   std::unordered_map<std::string, rsp_shard*> by_name;
   PinBuf pin_in, pin_out, pin_up, pin_totals;
-  DevBuf dev_tick, dev_q, dev_pending, dev_ops, dev_up;
+  DevBuf dev_tick, dev_q, dev_pending, dev_up;
   cudaEvent_t pending_ev = nullptr;  // the last device-form MultiGet launch (the pending list is per engine)
   bool pending_ev_recorded = false;
   cudaStream_t pending_last_stream = nullptr;
@@ -264,8 +264,6 @@ struct rsp_engine {
   ShardFast* d_fast_runs = nullptr;
   u32* d_mt_filter = nullptr;  // behind d_fast_runs in the same allocation (format.cuh: memtable filter)
   std::atomic<u32> n_multirun{0};
-  bool fused_ticks = true;  // RSP_FUSED_TICK=0: always the four general kernels (k_decode .. k_publish)
-  bool bg_compaction = true;  // RSP_BG_COMPACT=0: merges run on the apply path (r01 behaviour)
   struct Compactor* compactor = nullptr;
   u32 mg_parity = 0;
   size_t pending_cap = 0;
@@ -299,9 +297,6 @@ static void reader_end(rsp_engine* e, cudaStream_t s) {
   e->readers.note(s);
 }
 
-// runs_only: only the run set changed (a background merge was installed).  The sequencing state of the descriptor
-// (last_seq, pub_seq, mt_tail, mt_count, latch) belongs to the DEVICE while ticks are in flight — the host mirror may
-// lag behind pre-staged ticks — so it is not written then.
 // host bookkeeping + the compact descriptors of a shard (ShardFast, one per run) from its run list
 static void describe_shard(rsp_engine* e, rsp_shard* s, ShardFast* f_out, ShardFast* fr) {
   s->h.n_runs = (u32)s->runs.size();
@@ -329,24 +324,13 @@ static void describe_shard(rsp_engine* e, rsp_shard* s, ShardFast* f_out, ShardF
   f.merge_op = s->h.merge_op;
   *f_out = f;
 }
-static void upload_shard(rsp_engine* e, rsp_shard* s, bool runs_only = false) {
-  ShardFast f, fr[RSP_MAX_RUNS];
-  describe_shard(e, s, &f, fr);
-  if (runs_only) {
-    const size_t from = offsetof(ShardDev, n_runs);
-    CUDA_OK(cudaMemcpyAsync((u8*)(e->d_shards + s->index) + from, (const u8*)&s->h + from, sizeof(ShardDev) - from,
-                            cudaMemcpyHostToDevice, e->st));
-  } else {
-    CUDA_OK(cudaMemcpyAsync(e->d_shards + s->index, &s->h, sizeof(ShardDev), cudaMemcpyHostToDevice, e->st));
-  }
-  CUDA_OK(cudaMemcpyAsync(e->d_fast_runs + (size_t)s->index * RSP_MAX_RUNS, fr, sizeof(fr), cudaMemcpyHostToDevice, e->st));
-  // (runs_only: the first 24 bytes = run 0 + meta; mt_count is written by the sequencing kernels)
-  CUDA_OK(cudaMemcpyAsync(e->d_fast + s->index, &f, runs_only ? offsetof(ShardFast, mt_count) : sizeof(f), cudaMemcpyHostToDevice, e->st));
-  // the host mirror is pageable: the copy above is staged before the call returns
-}
-// The same for a batch of shards (a flush / merge batch installs up to thousands of descriptors): records staged in
-// pinned memory, one copy, one launch (k_upload_shards) — three pageable copies and a memset per shard cost the
-// install of a 1024-shard flush tens of milliseconds of driver calls.
+// A shard's descriptors reach the device only as a batch of upload records (a flush / merge batch installs up to
+// thousands of them): staged in pinned memory, one copy, one launch (k_upload_shards) — three pageable copies and a
+// memset per shard cost the install of a 1024-shard flush tens of milliseconds of driver calls.
+// runs_only: only the run set changed (a background merge was installed).  The sequencing state of the descriptor
+// (last_seq, pub_seq, mt_tail, mt_count, latch) belongs to the DEVICE while ticks are in flight — the host mirror may
+// lag behind pre-staged ticks — so it is not written then.  zero_mt: the memtable is empty (flushed or newly
+// allocated): its slot table and filter row are cleared.
 struct UploadBatch {
   std::vector<ShardUpload> recs;
 };
@@ -380,7 +364,8 @@ static u32 next_pow2(u32 x) {
   return p;
 }
 
-// (re)allocate an empty memtable able to hold at least `units` heap units and `ents` entries
+// (re)allocate an empty memtable able to hold at least `units` heap units and `ents` entries; the caller installs it
+// with a zero_mt upload record, which clears its slot table and filter row
 static void alloc_memtable(rsp_engine* e, rsp_shard* s, u64 units, u64 ents) {
   Arena& a = e->arena;
   if (s->h.mt_heap) {
@@ -392,7 +377,7 @@ static void alloc_memtable(rsp_engine* e, rsp_shard* s, u64 units, u64 ents) {
   }
   u64 want_units = std::max<u64>(units, (s->opts.write_buffer_bytes ? s->opts.write_buffer_bytes : (1u << 20)) / 16);
   u64 want_ents = std::max<u64>(ents, want_units / 7);  // a 16 B/64 B Put is 7 units
-  u32 slot_cap = next_pow2((u32)std::max<u64>(16, want_ents * 2));
+  u32 slot_cap = next_pow2((u32)std::max<u64>(16, want_ents * 2));  // (k_upload_shards clears >= 16 slots)
   s->mt_heap_bytes = want_units * 16;
   s->mt_slot_bytes = (size_t)slot_cap * 8;
   s->mt_ent_bytes = want_ents * 4;
@@ -404,8 +389,6 @@ static void alloc_memtable(rsp_engine* e, rsp_shard* s, u64 units, u64 ents) {
   s->h.mt_ent_cap = (u32)want_ents;
   s->h.mt_tail = 0;
   s->h.mt_count = 0;
-  CUDA_OK(cudaMemsetAsync(s->h.mt_slots, 0, s->mt_slot_bytes, e->st));
-  CUDA_OK(cudaMemsetAsync(e->d_mt_filter + (size_t)s->index * MT_FILTER_WORDS, 0, MT_FILTER_WORDS * 4, e->st));
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -475,15 +458,9 @@ static void plan_jobs(rsp_engine* e, const std::vector<rsp_shard*>& shards, Comp
       if (s->merging || s->runs.size() < e->cfg.l0_compaction_trigger) continue;
       n_merged = tiered_set(s, 0, s->runs.size(), false);
       if (n_merged < 2) continue;
-    } else if (mode == COMPACT_FLUSH) {
-      const bool table_full = s->runs.size() + 1 > RSP_MAX_RUNS - 1;
-      if (!e->bg_compaction) {
-        if (s->runs.size() + (has_mem ? 1 : 0) >= e->cfg.l0_compaction_trigger || table_full)
-          n_merged = tiered_set(s, has_mem ? (u64)s->h.mt_tail * 16 : 0, avail, table_full);
-      } else if (table_full) {
-        // merges belong to the background thread; the foreground only merges when the run table itself fills up
-        n_merged = tiered_set(s, has_mem ? (u64)s->h.mt_tail * 16 : 0, avail, true);
-      }
+    } else if (mode == COMPACT_FLUSH && s->runs.size() + 1 > RSP_MAX_RUNS - 1) {
+      // merges belong to the background thread; the foreground only merges when the run table itself fills up
+      n_merged = tiered_set(s, has_mem ? (u64)s->h.mt_tail * 16 : 0, avail, true);
     }
     // the run table must never overflow: if the flush would, everything is merged right here (a background merge of
     // some of these runs then finds its sources gone at install time and drops its output)
@@ -669,7 +646,7 @@ static void install_jobs(rsp_engine* e, CompactPlan* plan, CompactMode mode) {
   e->last_ms["compact_total"] += plan->ms;  // kernels of every flush / merge so far (sizing round trip included)
   for (u32 i = 0; i < nj; i++) {
     rsp_shard* s = plan->jh[i].s;
-    if (s && e->bg_compaction && s->runs.size() >= e->cfg.l0_compaction_trigger && !s->merging) bg_request(e, s);
+    if (s && s->runs.size() >= e->cfg.l0_compaction_trigger && !s->merging) bg_request(e, s);
   }
 }
 
@@ -969,7 +946,7 @@ static int stage_build(rsp_engine* e, size_t n, const uint32_t* shard_ix, const 
       BatchDesc& b = bd[pos];
       const u32 g = g_of[i];
       b.shard_ix = gd[g].shard_ix; b.boff = p_boff[pos]; b.len = (u32)len_eff;
-      b.op_base = p_opbase[pos]; b.op_cap = p_cap[pos]; b.group = g; b.raw_len = (u32)len_eff; b.pad1 = 0;
+      b.op_base = p_opbase[pos]; b.op_cap = p_cap[pos]; b.group = g; b.pad0 = 0; b.pad1 = 0;
       reinterpret_cast<u64*>(pin + o_foff)[pos] = p_boff[pos];
       reinterpret_cast<u32*>(pin + o_flen)[pos] = (u32)len_eff;
     }
@@ -1014,7 +991,6 @@ static int stage_build(rsp_engine* e, size_t n, const uint32_t* shard_ix, const 
   }
   CUDA_OK(cudaMemcpyAsync(dev, pin, in_b, cudaMemcpyHostToDevice, e->st));
   TickDev& t = sg->tick;
-  t.ts = nullptr;  // the LogData record is physically in the staged blob
   t.batches = (const BatchDesc*)dev;
   t.groups = (const GroupDesc*)(dev + n * sizeof(BatchDesc));
   t.blob = dev + desc_b;
@@ -1031,7 +1007,7 @@ static int stage_build(rsp_engine* e, size_t n, const uint32_t* shard_ix, const 
     size_t max_len = 0, max_group = 0;
     for (size_t i = 0; i < n; i++) max_len = std::max<size_t>(max_len, (size_t)(off[i + 1] - off[i]) + trailer);
     for (size_t g = 0; g < ng; g++) max_group = std::max<size_t>(max_group, g_count[g]);
-    sg->fused = e->fused_ticks && max_len <= FUSED_MAX_BATCH_BYTES;
+    sg->fused = max_len <= FUSED_MAX_BATCH_BYTES;
     FusedTick& f = sg->ftick;
     f.blob = t.blob; f.off = (const u64*)(dev + o_foff); f.len = (const u32*)(dev + o_flen); f.ts = nullptr;
     f.groups = t.groups; f.bstat = t.bstat; f.gres = t.gres; f.n_groups = (u32)ng; f.n_batches = (u32)n;
@@ -1079,15 +1055,22 @@ static int reserve_for(rsp_engine* e, const rsp_staged* sg) {
     if (s->h.mt_count) to_flush.push_back(s);
   }
   if (!to_flush.empty()) { compact_shards(e, to_flush, false); did_work = true; }
-  for (size_t g = 0; g < sg->group_shard.size(); g++) {
-    rsp_shard* s = sg->group_shard[g];
-    const u64 nu = sg->need_units[g], ne = sg->need_ents[g];
-    if (!fits(s, nu, ne)) {  // empty but too small for this tick
-      alloc_memtable(e, s, nu + nu / 2, ne + ne / 2);
-      upload_shard(e, s);
-      did_work = true;
+  UploadBatch up;
+  try {
+    for (size_t g = 0; g < sg->group_shard.size(); g++) {
+      rsp_shard* s = sg->group_shard[g];
+      const u64 nu = sg->need_units[g], ne = sg->need_ents[g];
+      if (!fits(s, nu, ne)) {  // empty but too small for this tick
+        alloc_memtable(e, s, nu + nu / 2, ne + ne / 2);
+        stage_upload(e, s, false, true, &up);
+        did_work = true;
+      }
     }
+  } catch (...) {  // (out of device memory): the memtables re-sized so far are installed all the same
+    commit_uploads(e, &up);
+    throw;
   }
+  commit_uploads(e, &up);
   for (size_t g = 0; g < sg->group_shard.size(); g++) {
     sg->group_shard[g]->inflight_units += sg->need_units[g];
     sg->group_shard[g]->inflight_ents += sg->need_ents[g];
@@ -1111,8 +1094,14 @@ static void tick_launch(rsp_engine* e, rsp_staged* sg, cudaStream_t st) {
   e->launches += 4;
 }
 
-// fold a tick's results (per-shard state + one status word per batch) into the host mirrors
-static int tick_results(rsp_staged* sg, const u8* pout, int32_t* st_out) {
+// bring a tick's results (per-shard state + one status word per batch) back from the stream it was launched on,
+// record its kernel time and fold the results into the host mirrors
+static int tick_results(rsp_engine* e, rsp_staged* sg, cudaStream_t st, int32_t* st_out) {
+  u8* pout = (u8*)e->pin_out.get(sg->res_bytes);
+  CUDA_OK(cudaMemcpyAsync(pout, sg->tick.gres, sg->res_bytes, cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaStreamSynchronize(st));
+  float ms = 0;
+  if (cudaEventElapsedTime(&ms, e->ev0, e->ev1) == cudaSuccess) e->last_ms["apply"] = ms;
   unreserve(sg);  // the mirrors below now include this tick
   const size_t ng = sg->group_shard.size();
   const GroupRes* gr = (const GroupRes*)pout;
@@ -1149,14 +1138,42 @@ static int tick_results(rsp_staged* sg, const u8* pout, int32_t* st_out) {
   return worst;
 }
 
-// Packed tick: when the caller's batches are already grouped by shard (each shard's batches contiguous, in
-// order — what a per-shard aggregator produces), nothing is re-laid out on the host: the caller's blob, offsets and
-// timestamps go to the device as they are (four copies), k_prepare derives the descriptors there, and the
-// follower's LogData(timestamp) record is a VIRTUAL suffix the decode kernel synthesises.  Host work per batch: one
-// comparison.  Returns -1 when the input does not qualify (the general, host-staged path takes over).
-static int apply_many_locked(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* blob, const uint64_t* off,
-                             const uint64_t* ts_ms, int32_t* st_out, bool allow_packed = true);
+// every batch of a tick answers Busy: pre-staged ticks are still in flight on a shard whose memtable is full (the
+// caller folds them first)
+static int all_busy(size_t n, int32_t* st_out) {
+  if (st_out) for (size_t i = 0; i < n; i++) st_out[i] = RSP_BUSY;
+  return RSP_BUSY;
+}
 
+// launch a reserved tick on the engine stream and fold its results; t0: when building the tick began (RSP_TRACE)
+static int tick_run(rsp_engine* e, rsp_staged* sg, int32_t* st_out, const char* kind, double t0) {
+  const double t1 = now_us();
+  CUDA_OK(cudaEventRecord(e->ev0, e->st));
+  tick_launch(e, sg, e->st);
+  CUDA_OK(cudaEventRecord(e->ev1, e->st));
+  const int worst = tick_results(e, sg, e->st, st_out);
+  if (g_trace)
+    fprintf(stderr, "[rsp trace] apply_many(%s) n=%zu build %.0f us device+results %.0f us (kernels %.0f us)\n", kind,
+            sg->n, t1 - t0, now_us() - t1, e->last_ms["apply"] * 1e3);
+  return worst;
+}
+
+// Host-staged tick: any input (stage_build groups the batches by shard and appends the LogData record)
+static int apply_many_staged(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* blob, const uint64_t* off,
+                             const uint64_t* ts_ms, int32_t* st_out) {
+  rsp_staged sg;
+  const double t0 = now_us();
+  const int rc = stage_build(e, n, shard_ix, blob, off, ts_ms, &sg, false);
+  if (rc != RSP_OK) return rc;
+  if (reserve_for(e, &sg) < 0) return all_busy(n, st_out);
+  return tick_run(e, &sg, st_out, "staged", t0);
+}
+
+// Packed tick: when the caller's batches are already grouped by shard (each shard's batches contiguous, in
+// order — what a per-shard aggregator produces) and small enough for the fused kernels, nothing is re-laid out on the
+// host: the caller's blob, offsets and timestamps go to the device as they are, and the follower's LogData(timestamp)
+// record is a VIRTUAL suffix the fused kernel synthesises.  Host work per batch: one comparison.  Returns -1 when the
+// input does not qualify (the host-staged path takes over).
 static int apply_many_packed(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* blob, const uint64_t* off,
                              const uint64_t* ts_ms, int32_t* st_out) {
   if (n < 1024 || off[0] != 0 || off[n] > 0xe0000000ull) return -1;
@@ -1182,23 +1199,19 @@ static int apply_many_packed(rsp_engine* e, size_t n, const uint32_t* shard_ix, 
     max_len = std::max<size_t>(max_len, (size_t)(off[i + 1] - off[i]));
   }
   for (const GroupDesc& g : groups) { seen[g.shard_ix] = 0; max_group = std::max<size_t>(max_group, g.n_batches); }
-  if (!ok) return -1;
-  const size_t ng = groups.size();
   const size_t trailer = ts_ms ? 10 : 0;
+  if (!ok || max_len + trailer > FUSED_MAX_BATCH_BYTES) return -1;
+  const size_t ng = groups.size();
   sg.group_first.resize(ng + 1);
   for (size_t g = 0; g < ng; g++) sg.group_first[g] = groups[g].first_batch;
   sg.group_first[ng] = (u32)n;
   const size_t blob_b = (size_t)off[n];
-  const bool fused = e->fused_ticks && max_len + trailer <= FUSED_MAX_BATCH_BYTES;
-  // device image: [groups][off][ts][need | total][BatchDesc][blob + slack][BatchRes][GroupRes | status]
-  // (the fused tick needs neither the descriptors nor the per-batch results: those regions are empty then)
+  // device image: [groups][off][ts][blob + slack][GroupRes | status]
   const size_t o_groups = 0, o_off = align_up(ng * sizeof(GroupDesc), 256), o_ts = o_off + align_up((n + 1) * 8, 256);
-  const size_t o_need = o_ts + align_up(n * 8, 256), o_desc = o_need + align_up((2 * ng + 1) * 4, 256);
-  const size_t o_blob = o_desc + (fused ? 0 : align_up(n * sizeof(BatchDesc), 256)), o_bres = o_blob + align_up(blob_b + 64, 256);
-  const size_t o_out = o_bres + (fused ? 0 : align_up(n * sizeof(BatchRes), 256));
+  const size_t o_blob = o_ts + align_up(n * 8, 256), o_out = o_blob + align_up(blob_b + 64, 256);
   // groups longer than one chunk: k_tick_chunks' chunk table, chain records and per-group counters
   std::vector<ChunkDesc> chunks;
-  if (fused && !fused_small_shape((u32)max_group, (u32)(max_len + trailer + 16)))
+  if (!fused_small_shape((u32)max_group, (u32)(max_len + trailer + 16)))
     cut_chunks(groups.data(), ng, [&](size_t i) { return (u64)off[i]; }, [&](size_t i) { return (u64)off[i + 1]; }, &chunks);
   const size_t o_chunks = o_out + align_up(ng * sizeof(GroupRes) + n * 4, 256);
   const size_t o_chain = o_chunks + align_up(chunks.size() * sizeof(ChunkDesc), 256);
@@ -1206,144 +1219,70 @@ static int apply_many_packed(rsp_engine* e, size_t n, const uint32_t* shard_ix, 
   sg.res_bytes = ng * sizeof(GroupRes) + n * 4;
   sg.need_units.resize(ng);
   sg.need_ents.resize(ng);
-  if (fused) {
-    // No sizing round trip: the memtable room is reserved from an ESTIMATE (bytes / 16 units of payload plus two
-    // header units per expected entry); the kernel's own capacity guard refuses what does not fit after all (status
-    // Busy, unlatched) and those batches are retried below through the general path, which reserves exact bounds.
-    for (size_t g = 0; g < ng; g++) {
-      const size_t first = groups[g].first_batch, nb = groups[g].n_batches;
-      const u64 bytes = off[first + nb] - off[first] + nb * trailer;
-      const u64 ents = nb + bytes / 256;
-      sg.need_ents[g] = (u32)ents;
-      sg.need_units[g] = (u32)(bytes / 16 + 2 * ents + 1);
-    }
-    if (reserve_for(e, &sg) < 0) {
-      if (st_out) for (size_t i = 0; i < n; i++) st_out[i] = RSP_BUSY;
-      return RSP_BUSY;
-    }
+  // No sizing round trip: the memtable room is reserved from an ESTIMATE (bytes / 16 units of payload plus two header
+  // units per expected entry); the kernel's own capacity guard refuses what does not fit after all (status Busy,
+  // unlatched) and those batches are retried below through the host-staged path, which reserves exact bounds.
+  for (size_t g = 0; g < ng; g++) {
+    const size_t first = groups[g].first_batch, nb = groups[g].n_batches;
+    const u64 bytes = off[first + nb] - off[first] + nb * trailer;
+    const u64 ents = nb + bytes / 256;
+    sg.need_ents[g] = (u32)ents;
+    sg.need_units[g] = (u32)(bytes / 16 + 2 * ents + 1);
   }
+  if (reserve_for(e, &sg) < 0) return all_busy(n, st_out);
   u8* dev = (u8*)e->dev_tick.get(total);
   CUDA_OK(cudaMemcpyAsync(dev + o_groups, groups.data(), ng * sizeof(GroupDesc), cudaMemcpyHostToDevice, e->st));
   CUDA_OK(cudaMemcpyAsync(dev + o_off, off, (n + 1) * 8, cudaMemcpyHostToDevice, e->st));
   if (ts_ms) CUDA_OK(cudaMemcpyAsync(dev + o_ts, ts_ms, n * 8, cudaMemcpyHostToDevice, e->st));
   CUDA_OK(cudaMemcpyAsync(dev + o_blob, blob, blob_b, cudaMemcpyHostToDevice, e->st));
   CUDA_OK(cudaMemsetAsync(dev + o_blob + blob_b, 0, 64, e->st));
-  u32* pneed = (u32*)e->pin_out.get((2 * ng + 1) * 4 + ng * sizeof(GroupRes) + n * 4 + 256);
-  u8* pout = (u8*)pneed + align_up((2 * ng + 1) * 4, 16);
-  double t1 = now_us();
-  if (fused) {
-    sg.fused = true;
-    FusedTick& f = sg.ftick;
-    f.blob = dev + o_blob; f.off = (const u64*)(dev + o_off); f.len = nullptr; f.ts = ts_ms ? (const u64*)(dev + o_ts) : nullptr;
-    f.groups = (const GroupDesc*)(dev + o_groups); f.gres = (GroupRes*)(dev + o_out);
-    f.bstat = (u32*)(dev + o_out + ng * sizeof(GroupRes)); f.n_groups = (u32)ng; f.n_batches = (u32)n;
-    f.max_group = (u32)max_group; f.max_len = (u32)(max_len + trailer + 16);
-    f.chunks = (const ChunkDesc*)(dev + o_chunks); f.n_chunks = (u32)chunks.size(); f.pad = 0;
-    f.chain = (u64*)(dev + o_chain); f.group_done = (u32*)(dev + o_chain + chunks.size() * 32);
-    if (!chunks.empty())
-      CUDA_OK(cudaMemcpyAsync(dev + o_chunks, chunks.data(), chunks.size() * sizeof(ChunkDesc), cudaMemcpyHostToDevice, e->st));
-    sg.tick.gres = f.gres;
-  } else {
-    CUDA_OK(cudaMemsetAsync(dev + o_need, 0, (2 * ng + 1) * 4, e->st));
-    PrepareArgs pa;
-    pa.blob = dev + o_blob; pa.off = (const u64*)(dev + o_off); pa.ts = ts_ms ? (const u64*)(dev + o_ts) : nullptr;
-    pa.groups = (const GroupDesc*)(dev + o_groups); pa.n_groups = (u32)ng; pa.n_batches = (u32)n;
-    pa.batches = (BatchDesc*)(dev + o_desc); pa.need = (u32*)(dev + o_need); pa.total_ops = (u32*)(dev + o_need) + 2 * ng;
-    launch_prepare(pa, e->st);
-    e->launches++;
-    CUDA_OK(cudaMemcpyAsync(pneed, dev + o_need, (2 * ng + 1) * 4, cudaMemcpyDeviceToHost, e->st));
-    CUDA_OK(cudaStreamSynchronize(e->st));
-    t1 = now_us();
-    for (size_t g = 0; g < ng; g++) { sg.need_units[g] = pneed[2 * g]; sg.need_ents[g] = pneed[2 * g + 1]; }
-    const u32 total_ops = pneed[2 * ng];
-    if (reserve_for(e, &sg) < 0) {
-      // pre-staged ticks are still in flight on these shards and the memtable is full: the caller folds them first
-      if (st_out) for (size_t i = 0; i < n; i++) st_out[i] = RSP_BUSY;
-      return RSP_BUSY;
-    }
-    TickDev& t = sg.tick;
-    t.blob = dev + o_blob; t.ts = pa.ts; t.batches = pa.batches; t.groups = pa.groups;
-    t.bres = (BatchRes*)(dev + o_bres); t.gres = (GroupRes*)(dev + o_out);
-    t.bstat = (u32*)(dev + o_out + ng * sizeof(GroupRes));
-    t.ops = (OpRec*)e->dev_ops.get((size_t)std::max<u32>(total_ops, 1) * sizeof(OpRec));
-    t.n_batches = (u32)n; t.n_groups = (u32)ng; t.n_ops_cap = total_ops;
-  }
-  CUDA_OK(cudaEventRecord(e->ev0, e->st));
-  tick_launch(e, &sg, e->st);
-  CUDA_OK(cudaEventRecord(e->ev1, e->st));
-  CUDA_OK(cudaMemcpyAsync(pout, sg.tick.gres, sg.res_bytes, cudaMemcpyDeviceToHost, e->st));
-  CUDA_OK(cudaStreamSynchronize(e->st));
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
-  e->last_ms["apply"] = ms;
-  const double t2 = now_us();
+  sg.fused = true;
+  FusedTick& f = sg.ftick;
+  f.blob = dev + o_blob; f.off = (const u64*)(dev + o_off); f.len = nullptr; f.ts = ts_ms ? (const u64*)(dev + o_ts) : nullptr;
+  f.groups = (const GroupDesc*)(dev + o_groups); f.gres = (GroupRes*)(dev + o_out);
+  f.bstat = (u32*)(dev + o_out + ng * sizeof(GroupRes)); f.n_groups = (u32)ng; f.n_batches = (u32)n;
+  f.max_group = (u32)max_group; f.max_len = (u32)(max_len + trailer + 16);
+  f.chunks = (const ChunkDesc*)(dev + o_chunks); f.n_chunks = (u32)chunks.size(); f.pad = 0;
+  f.chain = (u64*)(dev + o_chain); f.group_done = (u32*)(dev + o_chain + chunks.size() * 32);
+  if (!chunks.empty())
+    CUDA_OK(cudaMemcpyAsync(dev + o_chunks, chunks.data(), chunks.size() * sizeof(ChunkDesc), cudaMemcpyHostToDevice, e->st));
+  sg.tick.gres = f.gres;
   std::vector<int32_t> st_local;
-  if (fused && !st_out) { st_local.assign(n, 0); st_out = st_local.data(); }
-  int worst = tick_results(&sg, pout, st_out);
-  if (g_trace) fprintf(stderr, "[rsp trace] apply_many(packed%s) n=%zu copy%s %.0f us tick+sync %.0f us (kernels %.0f us) results %.0f us\n",
-                       fused ? ", fused" : "", n, fused ? "" : "+prepare", t1 - t0, t2 - t1, ms * 1e3, now_us() - t2);
-  if (fused) {
-    // batches the capacity guard refused (the estimate was too small for their shard): again, in order, with exact bounds
-    std::vector<uint32_t> again;
-    for (size_t i = 0; i < n; i++)
-      if (st_out[i] == RSP_BUSY && !e->slots[shard_ix[i]]->latch) again.push_back((uint32_t)i);
-    if (!again.empty()) {
-      const size_t m = again.size();
-      std::vector<uint32_t> six(m);
-      std::vector<uint64_t> off2(m + 1, 0), ts2(m);
-      std::vector<uint8_t> blob2;
-      for (size_t k = 0; k < m; k++) {
-        const size_t i = again[k];
-        six[k] = shard_ix[i];
-        blob2.insert(blob2.end(), blob + off[i], blob + off[i + 1]);
-        off2[k + 1] = blob2.size();
-        if (ts_ms) ts2[k] = ts_ms[i];
-      }
-      blob2.push_back(0);
-      std::vector<int32_t> st2(m, 0);
-      const int rc2 = apply_many_locked(e, m, six.data(), blob2.data(), off2.data(), ts_ms ? ts2.data() : nullptr, st2.data(), false);
-      for (size_t k = 0; k < m; k++) st_out[again[k]] = st2[k];
-      worst = RSP_OK;
-      for (size_t i = 0; i < n; i++) if (st_out[i]) { worst = st_out[i]; break; }
-      if (rc2 == RSP_BUSY) worst = RSP_BUSY;
+  if (!st_out) { st_local.assign(n, 0); st_out = st_local.data(); }
+  int worst = tick_run(e, &sg, st_out, "packed", t0);
+  // batches the capacity guard refused (the estimate was too small for their shard): again, in order, with exact bounds
+  std::vector<uint32_t> again;
+  for (size_t i = 0; i < n; i++)
+    if (st_out[i] == RSP_BUSY && !e->slots[shard_ix[i]]->latch) again.push_back((uint32_t)i);
+  if (!again.empty()) {
+    const size_t m = again.size();
+    std::vector<uint32_t> six(m);
+    std::vector<uint64_t> off2(m + 1, 0), ts2(m);
+    std::vector<uint8_t> blob2;
+    for (size_t k = 0; k < m; k++) {
+      const size_t i = again[k];
+      six[k] = shard_ix[i];
+      blob2.insert(blob2.end(), blob + off[i], blob + off[i + 1]);
+      off2[k + 1] = blob2.size();
+      if (ts_ms) ts2[k] = ts_ms[i];
     }
+    blob2.push_back(0);
+    std::vector<int32_t> st2(m, 0);
+    const int rc2 = apply_many_staged(e, m, six.data(), blob2.data(), off2.data(), ts_ms ? ts2.data() : nullptr, st2.data());
+    for (size_t k = 0; k < m; k++) st_out[again[k]] = st2[k];
+    worst = RSP_OK;
+    for (size_t i = 0; i < n; i++) if (st_out[i]) { worst = st_out[i]; break; }
+    if (rc2 == RSP_BUSY) worst = RSP_BUSY;
   }
   return worst;
 }
 
 static int apply_many_locked(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* blob,
-                             const uint64_t* off, const uint64_t* ts_ms, int32_t* st_out, bool allow_packed) {
+                             const uint64_t* off, const uint64_t* ts_ms, int32_t* st_out) {
   if (n == 0) return RSP_OK;
-  if (allow_packed && !getenv("RSP_NO_PACKED")) {
-    const int prc = apply_many_packed(e, n, shard_ix, blob, off, ts_ms, st_out);
-    if (prc >= 0) return prc;
-  }
-  rsp_staged sg;
-  // reserve first (may flush), then stage: staging uses the engine's tick buffers
-  // sizes are only known after grouping, so build the grouping twice is avoided by staging first into
-  // pinned memory and reserving before the H2D copy is consumed (same stream => ordered)
-  const double t0 = now_us();
-  int rc = stage_build(e, n, shard_ix, blob, off, ts_ms, &sg, false);
-  if (rc != RSP_OK) return rc;
-  const double t1 = now_us();
-  if (reserve_for(e, &sg) < 0) {
-    // pre-staged ticks are still in flight on these shards and the memtable is full: the caller folds them first
-    if (st_out) for (size_t i = 0; i < n; i++) st_out[i] = RSP_BUSY;
-    return RSP_BUSY;
-  }
-  CUDA_OK(cudaEventRecord(e->ev0, e->st));
-  tick_launch(e, &sg, e->st);
-  CUDA_OK(cudaEventRecord(e->ev1, e->st));
-  u8* pout = (u8*)e->pin_out.get(sg.res_bytes);
-  CUDA_OK(cudaMemcpyAsync(pout, sg.tick.gres, sg.res_bytes, cudaMemcpyDeviceToHost, e->st));
-  CUDA_OK(cudaStreamSynchronize(e->st));
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
-  e->last_ms["apply"] = ms;
-  const double t2 = now_us();
-  const int worst = tick_results(&sg, pout, st_out);
-  if (g_trace) fprintf(stderr, "[rsp trace] apply_many n=%zu stage %.0f us device+sync %.0f us (kernels %.0f us) results %.0f us\n", n, t1 - t0, t2 - t1, ms * 1e3, now_us() - t2);
-  return worst;
+  const int prc = apply_many_packed(e, n, shard_ix, blob, off, ts_ms, st_out);
+  if (prc >= 0) return prc;
+  return apply_many_staged(e, n, shard_ix, blob, off, ts_ms, st_out);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -2070,8 +2009,6 @@ int rsp_engine_create(int device, const rsp_engine_cfg* cfg, rsp_engine** out) {
   // two staging threads: more cost more in thread spawns than they save in copies
   e->stage_threads = 2;
   if (const char* t = getenv("RSP_STAGE_THREADS")) e->stage_threads = (size_t)std::max(1, atoi(t));
-  if (const char* t = getenv("RSP_FUSED_TICK")) e->fused_ticks = atoi(t) != 0;
-  if (const char* t = getenv("RSP_BG_COMPACT")) e->bg_compaction = atoi(t) != 0;
   CUDA_OK(cudaStreamCreateWithFlags(&e->st, cudaStreamNonBlocking));
   for (int k = 0; k < 3; k++) {
     CUDA_OK(cudaStreamCreateWithFlags(&e->cs[k], cudaStreamNonBlocking));
@@ -2093,7 +2030,7 @@ int rsp_engine_create(int device, const rsp_engine_cfg* cfg, rsp_engine** out) {
     e->d_fast_runs = e->d_fast + e->cfg.max_shards;
     e->d_mt_filter = reinterpret_cast<u32*>(e->d_fast + n_fast);
   }
-  if (e->bg_compaction) {
+  {
     Compactor* c = new Compactor();
     c->e = e;
     CUDA_OK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
@@ -2134,7 +2071,7 @@ void rsp_engine_destroy(rsp_engine* e) {
   for (rsp_shard* s : e->slots)
     if (s) { s->runs.clear(); delete s; }
   e->arena.destroy();
-  e->pin_in.destroy(); e->pin_out.destroy(); e->pin_up.destroy(); e->pin_totals.destroy(); e->dev_up.destroy(); e->dev_tick.destroy(); e->dev_q.destroy(); e->dev_pending.destroy(); e->dev_ops.destroy();
+  e->pin_in.destroy(); e->pin_out.destroy(); e->pin_up.destroy(); e->pin_totals.destroy(); e->dev_up.destroy(); e->dev_tick.destroy(); e->dev_q.destroy(); e->dev_pending.destroy();
   cudaFree(e->d_shards);
   cudaFree(e->d_fast);
   cudaEventDestroy(e->ev0); cudaEventDestroy(e->ev1); cudaEventDestroy(e->up_ev); cudaEventDestroy(e->pending_ev);
@@ -2164,7 +2101,9 @@ static int shard_open_locked(rsp_engine* e, const char* name, const rsp_shard_op
   s->h.merge_op = s->opts.merge_op;
   s->h.live = 1;
   alloc_memtable(e, s, 0, 0);
-  upload_shard(e, s);
+  UploadBatch up;
+  stage_upload(e, s, false, true, &up);
+  commit_uploads(e, &up);
   CUDA_OK(cudaStreamSynchronize(e->st));
   e->slots[ix] = s;
   e->by_name[name] = s;
@@ -2315,7 +2254,9 @@ int rsp_ingest_sorted(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_
       s->h.pub_seq = seq;
       s->last_seq.store(seq, std::memory_order_release);
     }
-    upload_shard(e, s);
+    UploadBatch up;
+    stage_upload(e, s, false, false, &up);
+    commit_uploads(e, &up);
     note_mutation(e);
     CUDA_OK(cudaStreamSynchronize(e->st));
   }
@@ -2340,7 +2281,9 @@ int rsp_set_latest_seq(rsp_shard* s, uint64_t seq) {
   s->h.last_seq = seq;
   s->h.pub_seq = seq;
   s->last_seq.store(seq, std::memory_order_release);
-  upload_shard(e, s);
+  UploadBatch up;
+  stage_upload(e, s, false, false, &up);
+  commit_uploads(e, &up);
   note_mutation(e);
   CUDA_OK(cudaStreamSynchronize(e->st));
   return RSP_OK;
@@ -3166,13 +3109,7 @@ int rsp_apply_staged_finish(rsp_engine* e, rsp_staged* sg, int32_t* st_out) {
   if (!e || !sg) return RSP_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(e->mu);
   CUDA_OK(cudaSetDevice(e->device));
-  u8* pout = (u8*)e->pin_out.get(sg->res_bytes);
-  cudaStream_t st = sg->last_stream ? sg->last_stream : e->st;
-  CUDA_OK(cudaMemcpyAsync(pout, sg->tick.gres, sg->res_bytes, cudaMemcpyDeviceToHost, st));
-  CUDA_OK(cudaStreamSynchronize(st));
-  float ms = 0;
-  if (cudaEventElapsedTime(&ms, e->ev0, e->ev1) == cudaSuccess) e->last_ms["apply"] = ms;
-  return tick_results(sg, pout, st_out);
+  return tick_results(e, sg, sg->last_stream ? sg->last_stream : e->st, st_out);
   } catch (...) { return abi_caught(); }
 }
 

@@ -179,7 +179,7 @@ __device__ __forceinline__ WalkResult walk_batch(Cursor c, Sink&& sink) {
 // writes one OpRec per op
 __device__ __forceinline__ void decode_batch(const TickDev& t, const u32 warp, const u32 lane) {
   const BatchDesc bd = t.batches[warp];
-  Cursor c{t.blob + bd.boff, 12, bd.len, bd.raw_len, t.ts ? __ldg(t.ts + warp) : 0ull};
+  Cursor c{t.blob + bd.boff, 12, bd.len, bd.len, 0ull};  // (staged: the LogData record is in the blob)
   const WalkResult w = walk_batch(c, [&](u32 type, u32 koff, u32 klen, u32 voff, u32 vlen, u32 units, u32 found) {
     if (found < bd.op_cap && lane == 0) {
       OpRec r;
@@ -421,8 +421,8 @@ __global__ void __launch_bounds__(256) k_insert(TickDev t, ShardDev* shards, u32
   if (op.type == kTypeInvalid) return;
   const BatchRes br = t.bres[op.batch_ix];
   if (!br.accepted) return;
-  const BatchDesc bdx = t.batches[op.batch_ix];
-  ShardDev* sd = shards + bdx.shard_ix;
+  const u32 six = t.batches[op.batch_ix].shard_ix;
+  ShardDev* sd = shards + six;
   u8* heap = sd->mt_heap;
   const u32 unit = br.unit_base + op.rel_units;
   const u64 seq = br.seq_base + op.op_ix;
@@ -430,33 +430,10 @@ __global__ void __launch_bounds__(256) k_insert(TickDev t, ShardDev* shards, u32
   u8* ent = heap + (u64)unit * 16u;
   u8* kdst = ent + 32u;
   u8* vdst = kdst + 16u * units_of(op.klen);
-  // A record whose key or value reaches into the VIRTUAL LogData bytes of a packed tick (a truncated batch
-  // that still parses, SURVEY §9 "swallow") is assembled byte by byte; everything else is word copies.
-  const u32 raw_end = bdx.boff + bdx.raw_len;
-  const bool crosses = op.koff + op.klen > raw_end || op.voff + op.vlen > raw_end;
-  u64 h;
-  if (!crosses) {
-    const u8* kp = t.blob + op.koff;
-    h = hash_key(kp, op.klen);  // every lane (redundant but free: the loads broadcast)
-    copy_to_units(kdst, kp, op.klen, lane, INS_LANES);
-    copy_to_units(vdst, t.blob + op.voff, op.vlen, lane, INS_LANES);
-  } else {
-    const u8* base = t.blob + bdx.boff;
-    const u64 ts = t.ts ? t.ts[op.batch_ix] : 0ull;
-    const u32 kpad = units_of(op.klen) * 16u, vpad = units_of(op.vlen) * 16u;
-    for (u32 b = lane; b < kpad; b += INS_LANES)
-      kdst[b] = b < op.klen ? (u8)batch_byte(base, bdx.raw_len, ts, op.koff - bdx.boff + b) : (u8)0;
-    for (u32 b = lane; b < vpad; b += INS_LANES)
-      vdst[b] = b < op.vlen ? (u8)batch_byte(base, bdx.raw_len, ts, op.voff - bdx.boff + b) : (u8)0;
-    __threadfence();
-    __syncwarp(gmask);
-    h = 0;
-    if (lane <= 1) {  // lanes 0 and 1 need the hash: recompute it from the padded heap copy
-      u64 hh = hash_init(op.klen);
-      for (u32 i = 0; i < ((op.klen + 7u) >> 3); i++) hh = hash_step(hh, ld_cg_u64(reinterpret_cast<const u64*>(kdst) + i));
-      h = hash_final(hh);
-    }
-  }
+  const u8* kp = t.blob + op.koff;
+  const u64 h = hash_key(kp, op.klen);  // every lane (redundant but free: the loads broadcast)
+  copy_to_units(kdst, kp, op.klen, lane, INS_LANES);
+  copy_to_units(vdst, t.blob + op.voff, op.vlen, lane, INS_LANES);
   if (lane == 0) {
     uint4 hd;
     const u64 st = (seq << 8) | op.type;
@@ -467,7 +444,7 @@ __global__ void __launch_bounds__(256) k_insert(TickDev t, ShardDev* shards, u32
   if (lane == 1) *reinterpret_cast<uint4*>(ent + 16) = make_uint4(0u, 0u, (u32)h, (u32)(h >> 32));
   u64* slots = sd->mt_slots;
   const u32 mask = sd->mt_slot_mask;
-  if (lane == 0) mt_filter_set(mt_filter + (size_t)bdx.shard_ix * MT_FILTER_WORDS, h);
+  if (lane == 0) mt_filter_set(mt_filter + (size_t)six * MT_FILTER_WORDS, h);
   const u64 first = lane == 0 ? ld_cg_u64(slots + ((u32)h & mask)) : 0ull;
   __threadfence();  // the entry is complete before any pointer to it is published
   __syncwarp(gmask);
@@ -859,43 +836,6 @@ void launch_tick_fused(const FusedTick& t, ShardDev* shards, ShardFast* fast, u3
     cudaMemsetAsync(t.chain, 0, (size_t)t.n_chunks * 32 + (size_t)t.n_groups * 4, s);
     k_tick_chunks<<<t.n_chunks, TC_THREADS, 0, s>>>(t, shards, fast, mt_filter);
   }
-}
-
-// ------------------------------------------------------------------------------------------------
-// k_prepare — packed ticks: BatchDesc straight from the caller's arrays (no host re-layout of the blob)
-// ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(256) k_prepare(PrepareArgs a) {
-  const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= a.n_batches) return;
-  // group of batch i: last group whose first_batch <= i
-  u32 lo = 0, hi = a.n_groups;
-  while (hi - lo > 1) {
-    const u32 m = (lo + hi) >> 1;
-    if (__ldg(&a.groups[m].first_batch) <= i) lo = m; else hi = m;
-  }
-  const u64 o0 = __ldg(a.off + i), o1 = __ldg(a.off + i + 1);
-  const u32 raw_len = (u32)(o1 - o0);
-  const u32 len_eff = raw_len + (a.ts ? 10u : 0u);
-  const u64 ts = a.ts ? __ldg(a.ts + i) : 0ull;
-  u32 claimed = 0;
-  if (len_eff >= 12) {
-    const u8* p = a.blob + o0;
-    claimed = batch_byte(p, raw_len, ts, 8) | (batch_byte(p, raw_len, ts, 9) << 8) | (batch_byte(p, raw_len, ts, 10) << 16) |
-              (batch_byte(p, raw_len, ts, 11) << 24);
-  }
-  const u32 max_ops = len_eff > 12 ? (len_eff - 12u) / 2u : 0u;
-  const u32 cap = min(claimed, max_ops);
-  BatchDesc b;
-  b.shard_ix = __ldg(&a.groups[lo].shard_ix);
-  b.boff = (u32)o0; b.len = len_eff; b.op_base = cap ? atomicAdd(a.total_ops, cap) : 0u; b.op_cap = cap; b.group = lo;
-  b.raw_len = raw_len; b.pad1 = 0;
-  a.batches[i] = b;
-  atomicAdd(a.need + 2 * lo, cap * 4u + len_eff / 16u + 1u);
-  atomicAdd(a.need + 2 * lo + 1, cap);
-}
-void launch_prepare(const PrepareArgs& a, cudaStream_t s) {
-  if (!a.n_batches) return;
-  k_prepare<<<(a.n_batches + 255) / 256, 256, 0, s>>>(a);
 }
 
 __global__ void k_publish(TickDev t, ShardDev* shards) {

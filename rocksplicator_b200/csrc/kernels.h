@@ -8,6 +8,8 @@ namespace rsp {
 constexpr u32 DEVICE_SMS = 132;
 
 // ---- apply tick image (device) -------------------------------------------------------------------
+// The general kernels (k_decode .. k_publish) take host-staged ticks only: every batch, its appended LogData(timestamp)
+// record included, is physically in the blob.
 struct BatchDesc {
   u32 shard_ix;
   u32 boff;    // byte offset of the batch in the tick blob
@@ -15,9 +17,7 @@ struct BatchDesc {
   u32 op_base; // first reserved slot in the op table
   u32 op_cap;  // reserved slots (min(header count, (len-12)/2))
   u32 group;
-  u32 raw_len; // bytes physically present in the blob; [raw_len, len) is the VIRTUAL LogData record
-               // {0x03, 0x08, timestamp LE} (packed ticks: nobody copies the batch to append it)
-  u32 pad1;
+  u32 pad0, pad1;
 };
 struct GroupDesc {
   u32 shard_ix;
@@ -52,7 +52,6 @@ struct __align__(16) OpRec {
 
 struct TickDev {
   const u8* blob;
-  const u64* ts;   // packed ticks: timestamp of batch i (virtual trailer); nullptr when the trailer is in the blob
   const BatchDesc* batches;
   const GroupDesc* groups;
   BatchRes* bres;
@@ -63,20 +62,6 @@ struct TickDev {
   u32 n_groups;
   u32 n_ops_cap;
 };
-
-// packed tick: descriptors are derived on the device from the caller's own arrays (no host re-layout)
-struct PrepareArgs {
-  const u8* blob;       // the caller's blob as given
-  const u64* off;       // [n+1]
-  const u64* ts;        // [n] or nullptr
-  const GroupDesc* groups;
-  u32 n_groups;
-  u32 n_batches;
-  BatchDesc* batches;   // out
-  u32* need;            // out [2 * n_groups]: upper bounds (heap units, entries) per group
-  u32* total_ops;       // out [1]
-};
-void launch_prepare(const PrepareArgs& a, cudaStream_t s);
 
 // the whole tick in one launch (ticks of small batches): batch i of group g is blob[off[i] .. off[i] + len[i]) (len ==
 // nullptr: the batches are contiguous, length off[i+1] - off[i]); ts != nullptr: the follower's LogData(timestamp)
