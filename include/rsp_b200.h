@@ -293,7 +293,10 @@ float rsp_last_kernel_ms(const rsp_engine* e, const char* what);
 /* number of engine kernels launched so far (bench.py's gpu_launches) */
 uint64_t rsp_kernel_launches(const rsp_engine* e);
 
-/* diagnostics: lookups of the last MultiGet launch that left the fast kernel for the generic path */
+/* diagnostics (synchronises the device): how many lookups of the engine's last host-form MultiGet that ran on the
+ * direct path (rsp_multi_get / rsp_multi_get_fixed) or last rsp_multi_get_device call the 16-byte-key kernel deferred
+ * to the generic path; their positions in that call's input, in no particular order, go to first[0 .. cap).  0 after
+ * a call the generic kernel served alone.  Requests the read combiner served are not covered. */
 uint32_t rsp_debug_last_pending(rsp_engine* e, uint32_t* first, uint32_t cap);
 
 /* diagnostics: the staging combiners' counters — which = 0 reads, 1 applies; out = {batches run, items carried,

@@ -267,6 +267,13 @@ struct rsp_engine {
   struct Compactor* compactor = nullptr;
   u32 mg_parity = 0;
   size_t pending_cap = 0;
+  // where the last host-form or device-form MultiGet left its deferred lookups (rsp_debug_last_pending): the
+  // 16-byte-key kernel ran (fast), the counter parity of a device-form launch, or the chunking of a host-form call
+  struct {
+    bool fast = false, host = false;
+    u32 parity = 0;
+    size_t n_chunks = 0, chunk = 0;
+  } last_mg;
   cudaEvent_t ev0 = nullptr, ev1 = nullptr;
   std::map<std::string, float> last_ms;
   std::atomic<u64> launches{0};
@@ -1430,6 +1437,8 @@ static int multi_get_locked(rsp_engine* e, size_t n, const uint32_t* shard_ix, c
   u32* scratch = (u32*)e->dev_pending.p;
   CUDA_OK(cudaMemsetAsync(scratch, 0, (4 + 2 * n_chunks) * 4, e->st));
   e->mg_parity = 0;
+  e->last_mg.fast = false; e->last_mg.host = true; e->last_mg.parity = 0;
+  e->last_mg.n_chunks = n_chunks; e->last_mg.chunk = CH;
   CUDA_OK(cudaEventRecord(e->ev0, e->st));
   for (size_t c = 0; c < n_chunks; c++) {
     const size_t c0 = c * CH, cn = piped ? std::min(CH, n - c0) : n;
@@ -1447,7 +1456,7 @@ static int multi_get_locked(rsp_engine* e, size_t n, const uint32_t* shard_ix, c
     a.vlen = (u32*)(d + o_vlen) + c0; a.st = (i32*)(d + o_st) + c0; a.n = (u32)cn;
     a.n_special = scratch; a.n_pending = scratch + 4 + 2 * c; a.pending = scratch + 4 + 2 * n_chunks + c0; a.parity = 0;
     a.multirun = e->n_multirun.load() ? 1u : 0u;
-    launch_multi_get(a, cs);
+    if (launch_multi_get(a, cs)) e->last_mg.fast = true;
     e->launches += 2;
     CUDA_OK(cudaMemcpyAsync(vlen + c0, d + o_vlen + c0 * 4, cn * 4, cudaMemcpyDeviceToHost, cs));
     CUDA_OK(cudaMemcpyAsync(st + c0, d + o_st + c0 * 4, cn * 4, cudaMemcpyDeviceToHost, cs));
@@ -3032,7 +3041,8 @@ int rsp_multi_get_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, co
     a.max_shards = e->cfg.max_shards;
     reader_begin(e, rs);
     a.multirun = e->n_multirun.load() ? 1u : 0u;
-    launch_multi_get(a, rs);
+    e->last_mg.fast = launch_multi_get(a, rs);
+    e->last_mg.host = false; e->last_mg.parity = a.parity; e->last_mg.n_chunks = 1; e->last_mg.chunk = n;
     reader_end(e, rs);
     pending_mark(e, rs);
   }
@@ -3144,16 +3154,37 @@ void rsp_debug_combiner_stats(rsp_engine* e, int which, uint64_t out[9]) {
   }
 }
 
-// diagnostics: how many lookups of the last MultiGet launch took the generic path (synchronises)
+// diagnostics: how many lookups of the last host-form or device-form MultiGet the 16-byte-key kernel deferred to the
+// generic path, and their positions in that call's input (synchronises).  The host form's scratch is
+// [n_special][pad][2 counters per chunk][one list per chunk, at the chunk's first lookup] with every counter at parity
+// 0; the device form's is [n_special][pad][2 counters, by launch parity][list].
 uint32_t rsp_debug_last_pending(rsp_engine* e, uint32_t* first, uint32_t cap) {
   try {
   std::lock_guard<std::mutex> g(e->mu);
   cudaSetDevice(e->device);
   cudaDeviceSynchronize();
-  if (!e->dev_pending.p) return 0;
+  if (!e->dev_pending.p || !e->last_mg.fast) return 0;
+  const u32* p = (const u32*)e->dev_pending.p;
+  const size_t nc = e->last_mg.n_chunks;
+  std::vector<u32> cnt(nc, 0);
+  if (e->last_mg.host) {
+    std::vector<u32> ctr(2 * nc);
+    cudaMemcpy(ctr.data(), p + 4, ctr.size() * 4, cudaMemcpyDeviceToHost);
+    for (size_t c = 0; c < nc; c++) cnt[c] = ctr[2 * c];
+  } else {
+    cudaMemcpy(cnt.data(), p + 2 + e->last_mg.parity, 4, cudaMemcpyDeviceToHost);
+  }
+  const u32* list = e->last_mg.host ? p + 4 + 2 * nc : p + 4;
   u32 n = 0;
-  cudaMemcpy(&n, (u32*)e->dev_pending.p + 2 + (e->mg_parity ^ 1u), 4, cudaMemcpyDeviceToHost);
-  if (first && cap) cudaMemcpy(first, (u32*)e->dev_pending.p + 4, 4 * std::min(n, cap), cudaMemcpyDeviceToHost);
+  for (size_t c = 0; c < nc; c++) {
+    const size_t c0 = c * e->last_mg.chunk;
+    const u32 take = first ? std::min<u32>(cnt[c], cap > n ? cap - n : 0u) : 0u;
+    if (take) {
+      cudaMemcpy(first + n, list + c0, 4 * (size_t)take, cudaMemcpyDeviceToHost);
+      for (u32 i = 0; i < take; i++) first[n + i] += (u32)c0;
+    }
+    n += cnt[c];
+  }
   return n;
   } catch (...) { abi_caught(); return 0; }
 }

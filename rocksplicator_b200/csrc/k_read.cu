@@ -280,8 +280,10 @@ __global__ void __launch_bounds__(256) k_multi_get(GetArgs a) {
 //      (2 lanes x 2 x 16 B = the 64-byte value)
 // The kernel is issue-bound before it is HBM-bound, so the lane count per lookup is what the instruction
 // budget allows: 8 lanes cost ~70 warp instructions per lookup, 2 lanes ~1/4 of that.
-// Anything else — tag false positive, probe longer than 4 buckets, Delete / Merge, version chains, several
-// runs, odd sizes — is appended to the pending list and served by the generic path (k_multi_get_pending).
+// Tag false positives and probes that spill past a full home bucket (wrapping at the last bucket) are served here
+// too.  Anything else — a memtable window with two tag matches or no empty slot, Delete / Merge, version chains,
+// several runs, entries of 255 units or more, values beyond the template's size — is appended to the pending list
+// and served by the generic path (k_multi_get_pending).
 static_assert(offsetof(ShardDev, mt_slot_mask) == 24 && offsetof(ShardDev, pub_seq) == 56, "ShardDev units 0-3");
 static_assert(sizeof(ShardFast) == 32, "ShardFast");
 
@@ -724,8 +726,8 @@ __global__ void __launch_bounds__(256) k_multi_get_pending(GetArgs a) {
     lookup_generic(a, __ldcg(a.pending + i), lane, gmask, gbase);
 }
 
-void launch_multi_get(const GetArgs& a, cudaStream_t s) {
-  if (!a.n) return;
+bool launch_multi_get(const GetArgs& a, cudaStream_t s) {
+  if (!a.n) return false;
   const u32 per_block = 256 / MG_LANES;
   const u32 grid = (a.n + per_block - 1) / per_block;
   if (a.klen_fixed == 16 && (reinterpret_cast<uintptr_t>(a.keys) & 15u) == 0 && a.pending && a.fast) {
@@ -741,9 +743,10 @@ void launch_multi_get(const GetArgs& a, cudaStream_t s) {
       if (multi) k_multi_get16m<false><<<g16, RSP_MG_TPB, 0, s>>>(a); else k_multi_get16<false><<<g16, RSP_MG_TPB, 0, s>>>(a);
     }
     k_multi_get_pending<<<std::min<u32>(grid, DEVICE_SMS), 256, 0, s>>>(a);
-  } else {
-    k_multi_get<<<grid, 256, 0, s>>>(a);
+    return true;
   }
+  k_multi_get<<<grid, 256, 0, s>>>(a);
+  return false;
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -129,7 +129,9 @@ struct GetArgs {
                          // register allocation of k_multi_get16 and slows it down)
 };
 static_assert(sizeof(GetArgs) == 128, "GetArgs layout is part of k_multi_get16's measured code generation");
-void launch_multi_get(const GetArgs& a, cudaStream_t s);
+// true when the 16-byte-key kernel ran (its deferred lookups are in a.pending, counted in a.n_pending[a.parity]);
+// false when the generic kernel served every lookup
+bool launch_multi_get(const GetArgs& a, cudaStream_t s);
 
 // dump the version stack of each key (newest first, up to and including the first Put/Delete) for
 // host-side merge folding: records [u32 type][u32 vlen][value, padded to 4] at out + i*stride

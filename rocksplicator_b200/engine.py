@@ -456,6 +456,13 @@ class Engine:
     def last_kernel_ms(self, what): return self.lib.rsp_last_kernel_ms(self.h, what.encode())
     def kernel_launches(self): return self.lib.rsp_kernel_launches(self.h)
 
+    def debug_last_pending(self, out=None):
+        """lookups of the last multi_get_fixed / rsp_multi_get_device call (not the read combiner's) that the 16-byte-key
+        kernel deferred to the generic path: returns their number and writes their positions (in no particular order)
+        into `out`, a uint32 array, up to its length"""
+        cap = 0 if out is None else len(out)
+        return self.lib.rsp_debug_last_pending(self.h, _ptr(out) if cap else None, cap)
+
 
 class Router:
     """Several engines (one per GPU) behind one handle: shard_id -> engine fan-out of cross-shard batches
