@@ -313,7 +313,7 @@ static void describe_shard(rsp_engine* e, rsp_shard* s, ShardFast* f_out, ShardF
   }
   auto describe = [](const Run& r, ShardFast* f) {
     f->run0_heap = (u64)r.heap; f->run0_hslots = (u64)r.hslots; f->n_buckets = r.n_buckets;
-    f->meta = r.ord_bits | (std::min<u32>(r.uniform_units, 255u) << 8);
+    f->meta = r.ord_bits | (std::min<u32>(r.uniform_units, 255u) << FAST_META_UNITS_SHIFT);
   };
   ShardFast f;
   memset(&f, 0, sizeof(f));
@@ -325,8 +325,8 @@ static void describe_shard(rsp_engine* e, rsp_shard* s, ShardFast* f_out, ShardF
     if (multi_now) e->n_multirun++; else e->n_multirun--;
     s->counted_multirun = multi_now;
   }
-  f.meta |= (u32)std::min<size_t>(s->runs.size(), 255) << 16;
-  f.meta |= 1u << 24;  // live
+  f.meta |= (u32)std::min<size_t>(s->runs.size(), 255) << FAST_META_RUNS_SHIFT;
+  f.meta |= FAST_META_LIVE;
   f.mt_count = s->h.mt_count;
   f.merge_op = s->h.merge_op;
   *f_out = f;
@@ -1409,6 +1409,49 @@ static void set_pending(rsp_engine* e, GetArgs& a, size_t n, cudaStream_t stream
   e->mg_parity ^= 1u;
 }
 
+// the fields of a MultiGet launch the engine owns: the shard descriptors, and whether some shard has several runs
+static void set_engine_args(rsp_engine* e, GetArgs& a) {
+  a.shards = e->d_shards; a.fast = e->d_fast; a.max_shards = e->cfg.max_shards;
+  a.multirun = e->n_multirun.load() ? 1u : 0u;
+}
+
+// statuses the fast / generic kernels settle themselves; anything else (host-folded merges, error texts, unknown
+// shards) is post-processed by the direct path
+static inline bool plain_status(int32_t st) { return st == RSP_OK || st == RSP_NOT_FOUND || st == RSP_INCOMPLETE; }
+
+// The statuses a MultiGet launch leaves to the host (the kernel counts them in n_special): ST_NEED_HOST_MERGE is
+// folded through the version dump and the shard's host operator, an error status turns the message id it carries in
+// vlen into the shard's error text.  ref(i) gives lookup i's shard (nullptr: unknown shard or snapshot, no text), key
+// and key length, and the pinned view it reads (nullptr: the live shard).
+struct LookupRef {
+  rsp_shard* s;
+  const uint8_t* key;
+  size_t klen;
+  const ScanView* d_view;
+};
+template <class Ref>
+static void finish_special(rsp_engine* e, size_t n, Ref ref, uint8_t* vals, size_t val_stride, uint32_t* vlen, int32_t* st) {
+  for (size_t i = 0; i < n; i++) {
+    if (plain_status(st[i])) continue;
+    const LookupRef r = ref(i);
+    if (st[i] == ST_NEED_HOST_MERGE) {
+      std::string v;
+      const int rc = host_fold_get(e, r.s, r.key, r.klen, &v, r.d_view);
+      st[i] = rc;
+      vlen[i] = 0;
+      if (rc == RSP_OK) {
+        vlen[i] = (u32)v.size();
+        if (v.size() > val_stride) st[i] = RSP_INCOMPLETE;
+        else memcpy(vals + i * val_stride, v.data(), v.size());
+      }
+    } else {
+      const u32 msg = vlen[i];
+      if (r.s) set_err(r.s, msg < MSG_COUNT ? kMsgText[msg] : "error");
+      vlen[i] = 0;
+    }
+  }
+}
+
 // One MultiGet over host buffers.  Large fixed-key batches are cut into chunks that ride three streams
 // (H2D -> kernel -> D2H per chunk), so the copy engines and the SMs overlap: the end-to-end rate is set by
 // the slower PCIe direction, not by the sum of both plus the kernel.
@@ -1449,13 +1492,12 @@ static int multi_get_locked(rsp_engine* e, size_t n, const uint32_t* shard_ix, c
     const size_t kb0 = klen_fixed ? c0 * klen_fixed : 0, kbn = klen_fixed ? cn * klen_fixed : key_bytes;
     if (kbn) CUDA_OK(cudaMemcpyAsync(d + o_keys + kb0, keys + kb0, kbn, cudaMemcpyHostToDevice, cs));
     GetArgs a;
-    a.shards = e->d_shards; a.fast = e->d_fast; a.max_shards = e->cfg.max_shards;
+    set_engine_args(e, a);
     a.shard_ix = (const u32*)(d + o_six) + c0; a.keys = d + o_keys + kb0;
     a.koff = klen_fixed ? nullptr : (const u64*)(d + o_koff); a.klen_fixed = klen_fixed;
     a.vals = d + o_vals + c0 * val_stride; a.val_stride = val_stride;
     a.vlen = (u32*)(d + o_vlen) + c0; a.st = (i32*)(d + o_st) + c0; a.n = (u32)cn;
     a.n_special = scratch; a.n_pending = scratch + 4 + 2 * c; a.pending = scratch + 4 + 2 * n_chunks + c0; a.parity = 0;
-    a.multirun = e->n_multirun.load() ? 1u : 0u;
     if (launch_multi_get(a, cs)) e->last_mg.fast = true;
     e->launches += 2;
     CUDA_OK(cudaMemcpyAsync(vlen + c0, d + o_vlen + c0 * 4, cn * 4, cudaMemcpyDeviceToHost, cs));
@@ -1476,28 +1518,12 @@ static int multi_get_locked(rsp_engine* e, size_t n, const uint32_t* shard_ix, c
   cudaEventElapsedTime(&ms, e->ev0, e->ev1);
   e->last_ms["multi_get"] = ms;
   if (!n_special) return RSP_OK;
-  // post-process the rare statuses: error texts, host-folded merges, unknown shards
-  for (size_t i = 0; i < n; i++) {
-    if (st[i] == ST_NEED_HOST_MERGE) {
-      rsp_shard* s = e->slots[shard_ix[i]];
-      const uint8_t* k = klen_fixed ? keys + i * klen_fixed : keys + koff[i];
-      const size_t kl = klen_fixed ? klen_fixed : (size_t)(koff[i + 1] - koff[i]);
-      std::string v;
-      int rc = host_fold_get(e, s, k, kl, &v);
-      st[i] = rc;
-      vlen[i] = 0;
-      if (rc == RSP_OK) {
-        vlen[i] = (u32)v.size();
-        if (v.size() > val_stride) st[i] = RSP_INCOMPLETE;
-        else memcpy(vals + i * val_stride, v.data(), v.size());
-      }
-    } else if (st[i] != RSP_OK && st[i] != RSP_NOT_FOUND && st[i] != RSP_INCOMPLETE) {
-      const u32 msg = vlen[i];
-      if (shard_ix[i] < e->slots.size() && e->slots[shard_ix[i]])
-        set_err(e->slots[shard_ix[i]], msg < MSG_COUNT ? kMsgText[msg] : "error");
-      vlen[i] = 0;
-    }
-  }
+  finish_special(e, n, [&](size_t i) {
+    const u32 six = shard_ix[i];
+    rsp_shard* s = six < e->slots.size() ? e->slots[six] : nullptr;
+    if (klen_fixed) return LookupRef{s, keys + i * klen_fixed, klen_fixed, nullptr};
+    return LookupRef{s, keys + koff[i], (size_t)(koff[i + 1] - koff[i]), nullptr};
+  }, vals, val_stride, vlen, st);
   return RSP_OK;
 }
 
@@ -1722,12 +1748,11 @@ struct ReadCombiner {
       if (info.n_bytes) CUDA_OK(cudaMemcpyAsync(S.dev + o_keys, S.pin + o_keys, info.n_bytes, cudaMemcpyHostToDevice, stream));
     }
     GetArgs a;
-    a.shards = e->d_shards; a.fast = e->d_fast; a.max_shards = e->cfg.max_shards;
+    set_engine_args(e, a);
     a.shard_ix = (const u32*)(base + o_six); a.keys = base + o_keys;
     a.koff = fixed16 ? nullptr : (const u64*)(base + o_koff); a.klen_fixed = fixed16 ? 16u : 0u;
     a.vals = base + o_vals; a.val_stride = stride; a.vlen = (u32*)(base + o_vlen); a.st = (i32*)(base + o_st); a.n = (u32)n;
     a.n_special = nullptr; a.n_pending = S.d_pending; a.pending = S.d_pending + 4; a.parity = 0;
-    a.multirun = e->n_multirun.load() ? 1u : 0u;
     {
       // ordering against flushes / memtable re-allocations on the engine stream (reader_begin / reader_end)
       std::lock_guard<std::mutex> g(e->mu);
@@ -2353,10 +2378,6 @@ int rsp_apply_updates(rsp_shard* s, size_t n, const rsp_slice* batches, const ui
   } catch (...) { return abi_caught(); }
 }
 
-// statuses the fast / generic kernels settle themselves; anything else (host-folded merges, error texts, unknown
-// shards) is post-processed by the direct path
-static inline bool plain_status(int32_t st) { return st == RSP_OK || st == RSP_NOT_FOUND || st == RSP_INCOMPLETE; }
-
 static int multi_get_direct(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
                             uint32_t klen_fixed, uint8_t* vals, size_t val_stride, uint32_t* vlen, int32_t* st) {
   std::lock_guard<std::mutex> g(e->mu);
@@ -2896,25 +2917,10 @@ static int multi_get_at_locked(rsp_engine* e, size_t n, rsp_snapshot* const* sna
   cudaEventElapsedTime(&ms, e->ev0, e->ev1);
   e->last_ms["multi_get_at"] = ms;
   if (!n_special) return RSP_OK;
-  for (size_t i = 0; i < n; i++) {
-    if (slot[i] == 0xffffffffu) continue;  // InvalidArgument, no text
-    rsp_shard* s = snaps[i]->s;
-    if (st[i] == ST_NEED_HOST_MERGE) {
-      std::string v;
-      const int rc = host_fold_get(e, s, keys + koff[i], (size_t)(koff[i + 1] - koff[i]), &v, e->d_snap_views + slot[i]);
-      st[i] = rc;
-      vlen[i] = 0;
-      if (rc == RSP_OK) {
-        vlen[i] = (u32)v.size();
-        if (v.size() > val_stride) st[i] = RSP_INCOMPLETE;
-        else memcpy(vals + i * val_stride, v.data(), v.size());
-      }
-    } else if (!plain_status(st[i])) {
-      const u32 msg = vlen[i];
-      set_err(s, msg < MSG_COUNT ? kMsgText[msg] : "error");
-      vlen[i] = 0;
-    }
-  }
+  finish_special(e, n, [&](size_t i) {
+    if (slot[i] == 0xffffffffu) return LookupRef{nullptr, nullptr, 0, nullptr};  // InvalidArgument, no text
+    return LookupRef{snaps[i]->s, keys + koff[i], (size_t)(koff[i + 1] - koff[i]), e->d_snap_views + slot[i]};
+  }, vals, val_stride, vlen, st);
   return RSP_OK;
 }
 
@@ -3032,15 +3038,14 @@ int rsp_multi_get_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, co
   try {
   if (!e || !klen) return RSP_INVALID_ARGUMENT;
   GetArgs a;
-  a.shards = e->d_shards; a.fast = e->d_fast; a.shard_ix = d_shard_ix; a.keys = d_keys; a.koff = nullptr; a.klen_fixed = klen;
+  a.shard_ix = d_shard_ix; a.keys = d_keys; a.koff = nullptr; a.klen_fixed = klen;
   a.vals = d_vals; a.val_stride = val_stride; a.vlen = d_vlen; a.st = d_st; a.n = (u32)n;
   {
     std::lock_guard<std::mutex> g(e->mu);  // the pending-list scratch is per engine
     cudaStream_t rs = stream ? (cudaStream_t)stream : e->st;
     set_pending(e, a, n, rs);
-    a.max_shards = e->cfg.max_shards;
     reader_begin(e, rs);
-    a.multirun = e->n_multirun.load() ? 1u : 0u;
+    set_engine_args(e, a);
     e->last_mg.fast = launch_multi_get(a, rs);
     e->last_mg.host = false; e->last_mg.parity = a.parity; e->last_mg.n_chunks = 1; e->last_mg.chunk = n;
     reader_end(e, rs);

@@ -107,7 +107,6 @@ struct __align__(16) RunDev {
   u32 kv_len;    // klen | vlen << 16 when RUN_ALL_PUT_FIXED
 };
 constexpr u32 RUN_ALL_PUT_FIXED = 1u;
-constexpr u32 FAST_META_LIVE = 1u << 24;
 
 struct __align__(16) ShardDev {
   // ---- memtable
@@ -135,10 +134,13 @@ struct __align__(32) ShardFast {
   u64 run0_heap;
   u64 run0_hslots;
   u32 n_buckets;
-  u32 meta;      // ord_bits | uniform_units << 8 | n_runs << 16
+  u32 meta;      // one byte each: ord_bits | uniform_units << 8 | n_runs << 16 | FAST_META_LIVE
   u32 mt_count;
   u32 merge_op;
 };
+constexpr u32 FAST_META_UNITS_SHIFT = 8;   // uniform_units, capped at 255 (0 and 255: the generic path)
+constexpr u32 FAST_META_RUNS_SHIFT = 16;   // the shard's run count, capped at 255 (per-run descriptors: 0)
+constexpr u32 FAST_META_LIVE = 1u << 24;   // the shard is open (per-run descriptors: 0)
 
 // ---- memtable filter -------------------------------------------------------------------------------
 // One bit per inserted key hash, MT_FILTER_BITS per shard, in one array behind the ShardFast descriptors (8 MB for 1024

@@ -172,20 +172,28 @@ __device__ __forceinline__ bool walk_run(const RunDev& r, const u8* kp, u32 klen
   return false;
 }
 
+// the sorted runs newest first, until the visitor is done.  n_runs is read before each run: a caller that wants it read
+// once passes a local copy.
+template <u32 G, class V>
+__device__ __forceinline__ void walk_runs(const RunDev* runs, const u32& n_runs, const u8* kp, u32 klen, u64 h, u32 lane,
+                                          u32 gmask, u32 gbase, V& v) {
+  for (u32 ri = 0; ri < n_runs && !v.done; ri++) walk_run<G>(runs[ri], kp, klen, h, lane, gmask, gbase, v);
+}
+
+// the memtable, then the sorted runs; the walk stops right after the visit that finishes
 template <u32 G, class V>
 __device__ __forceinline__ void walk_shard(const ShardDev* sd, const u8* kp, u32 klen, u32 lane, u32 gmask,
-                                           u32 gbase, V& v, bool& stopped) {
+                                           u32 gbase, V& v) {
   const u64 h = hash_key(kp, klen);
   const u64 snap = ldcg64(&sd->pub_seq);
-  stopped = false;
   if (ldcg32(&sd->mt_count) != 0) {
     walk_memtable<G>(sd, kp, klen, h, snap, lane, gmask, gbase, v);
-    if (v.done) { stopped = true; return; }
+    if (v.done) return;
   }
   const u32 n_runs = sd->n_runs;
   for (u32 ri = 0; ri < n_runs; ri++) {
     walk_run<G>(sd->runs[ri], kp, klen, h, lane, gmask, gbase, v);
-    if (v.done) { stopped = true; return; }
+    if (v.done) return;
   }
 }
 
@@ -205,34 +213,35 @@ __device__ __forceinline__ void group_copy_out(u8* dst, const u8* src, u32 n, u3
   }
 }
 
-// generic path: any key length, any entry shape, memtable chains, merges, multiple runs
-__device__ __noinline__ void lookup_generic(const GetArgs& a, u32 q, u32 lane, u32 gmask, u32 gbase) {
-  const u32 six = __ldg(a.shard_ix + q);
-  if (six >= a.max_shards || !a.shards[six].live) {  // unknown / closed shard
-    if (lane == 0) {
-      a.st[q] = 4;
-      a.vlen[q] = 0;
-      if (a.n_special) atomicAdd(a.n_special, 1u);
-    }
-    return;
-  }
-  const ShardDev* sd = a.shards + six;
-  const u8* kp;
-  u32 klen;
+// The eight-lane lookups of k_multi_get / k_multi_get_pending (GetArgs) and k_multi_get_at (GetAtArgs) share these
+// steps; both argument structs name the key and result fields alike.
+template <class Args>
+__device__ __forceinline__ const u8* lookup_key(const Args& a, u32 q, u32& klen) {
   if (a.klen_fixed) {
     klen = a.klen_fixed;
-    kp = a.keys + (u64)q * klen;
-  } else {
-    const u64 o = __ldg(a.koff + q);
-    klen = (u32)(__ldg(a.koff + q + 1) - o);
-    kp = a.keys + o;
+    return a.keys + (u64)q * klen;
   }
-  Acc acc;
-  acc.init(sd->merge_op);
-  bool stopped;
-  walk_shard<MG_LANES>(sd, kp, klen, lane, gmask, gbase, acc, stopped);
+  const u64 o = __ldg(a.koff + q);
+  klen = (u32)(__ldg(a.koff + q + 1) - o);
+  return a.keys + o;
+}
+
+// an unknown or closed shard, or a null, released or foreign snapshot: InvalidArgument
+template <class Args>
+__device__ __forceinline__ void answer_invalid(const Args& a, u32 q, u32 lane) {
+  if (lane == 0) {
+    a.st[q] = 4;
+    a.vlen[q] = 0;
+    if (a.n_special) atomicAdd(a.n_special, 1u);
+  }
+}
+
+// status, value and value length (the message id for error statuses) of a walk that has seen every version it needs
+template <class Args>
+__device__ __forceinline__ void answer(const Args& a, u32 q, u32 lane, Acc& acc) {
   acc.end_of_versions();
   i32 st = acc.status;
+  const u32 msg = acc.msg;
   u32 vlen = 0;
   if (st == 0) {
     vlen = acc.res_len;
@@ -250,13 +259,26 @@ __device__ __noinline__ void lookup_generic(const GetArgs& a, u32 q, u32 lane, u
       }
     }
   } else if (st != 1 && st != ST_NEED_HOST_MERGE) {
-    vlen = acc.msg;  // message id rides in vlen for error statuses
+    vlen = msg;  // message id rides in vlen for error statuses
   }
   if (lane == 0) {
     a.st[q] = st;
     a.vlen[q] = vlen;
     if (st != 0 && st != 1 && st != 7 && a.n_special) atomicAdd(a.n_special, 1u);
   }
+}
+
+// generic path: any key length, any entry shape, memtable chains, merges, multiple runs
+__device__ __noinline__ void lookup_generic(const GetArgs& a, u32 q, u32 lane, u32 gmask, u32 gbase) {
+  const u32 six = __ldg(a.shard_ix + q);
+  if (six >= a.max_shards || !a.shards[six].live) return answer_invalid(a, q, lane);
+  const ShardDev* sd = a.shards + six;
+  u32 klen;
+  const u8* kp = lookup_key(a, q, klen);
+  Acc acc;
+  acc.init(sd->merge_op);
+  walk_shard<MG_LANES>(sd, kp, klen, lane, gmask, gbase, acc);
+  answer(a, q, lane, acc);
 }
 
 __global__ void __launch_bounds__(256) k_multi_get(GetArgs a) {
@@ -270,7 +292,7 @@ __global__ void __launch_bounds__(256) k_multi_get(GetArgs a) {
 
 // Tried and dropped: hash-addressed entry slots instead of the index, and software prefetch of later lookups' sectors
 // (both slower than the index probe below).
-// ---- the hot kernel: 16-byte keys, TWO lanes per lookup, three dependent memory round trips ----------
+// ---- the hot kernels: 16-byte keys, TWO lanes per lookup, three dependent memory round trips ----------
 //   1. shard id + query key (coalesced across the warp) and the 32-byte ShardFast descriptor
 //      (32 B x #shards: L1/L2-resident); both lanes load the same words (one broadcast transaction)
 //   2. the hash bucket: one 32-byte sector of run 0's index, four u32 slots (one 16-byte load) per lane
@@ -278,38 +300,31 @@ __global__ void __launch_bounds__(256) k_multi_get(GetArgs a) {
 //   3. the entry: both lanes read the header and key units (same sector, broadcast) and decide alike with
 //      no shuffles; lane L then moves value units L, L+2, .. straight from its registers to the output
 //      (2 lanes x 2 x 16 B = the 64-byte value)
-// The kernel is issue-bound before it is HBM-bound, so the lane count per lookup is what the instruction
+// The kernels are issue-bound before they are HBM-bound, so the lane count per lookup is what the instruction
 // budget allows: 8 lanes cost ~70 warp instructions per lookup, 2 lanes ~1/4 of that.
 // Tag false positives and probes that spill past a full home bucket (wrapping at the last bucket) are served here
 // too.  Anything else — a memtable window with two tag matches or no empty slot, Delete / Merge, version chains,
-// several runs, entries of 255 units or more, values beyond the template's size — is appended to the pending list
-// and served by the generic path (k_multi_get_pending).
+// several runs (k_multi_get16), entries of 255 units or more, values beyond the template's size — is appended to the
+// pending list and served by the generic path (k_multi_get_pending).
 static_assert(offsetof(ShardDev, mt_slot_mask) == 24 && offsetof(ShardDev, pub_seq) == 56, "ShardDev units 0-3");
 static_assert(sizeof(ShardFast) == 32, "ShardFast");
 
 constexpr u32 FL = 2;  // lanes per lookup
+// 20 blocks of 64 threads per SM leave 48 registers per thread.  At 24 blocks (40 registers) ptxas for sm_90a spills
+// k_multi_get16<false> to local memory (60 bytes per thread), and the launch of 8.4 M lookups takes 1.04 ms instead of
+// 0.91 ms on an H100 80GB HBM3 at a 400 W power limit: the spill traffic costs more than the extra lookups in flight buy.
+constexpr u32 MG16_THREADS = 64;
+constexpr u32 MG16_MIN_BLOCKS = 20;
 
-// L2 residency control (createpolicy + ld/st .L2::cache_hint): the hash-index sectors are the only
-// data with reuse across lookups (80 MB at 10 M keys against a 50 MB L2); entries, query keys and results stream through once.  RSP_MG_HINTS: 0 = none, 1 = index evict_last, 2 = also
-// streams evict_first (an experiment switch).  RSP_MG_NOALLOC: entry units bypass L1.
-#ifndef RSP_MG_HINTS
-#define RSP_MG_HINTS 1
-#endif
+// L2 residency control (createpolicy + ld .L2::cache_hint): the hash-index sectors are the only data with reuse
+// across lookups (80 MB at 10 M keys against a 50 MB L2), so they are loaded evict_last; entries, query keys and
+// results stream through once.
 __device__ __forceinline__ u64 pol_evict_last() {
   u64 p;
 #ifdef RSP_EMUL  // tests/emul: cache policies have no meaning on the CPU
   p = 0;
 #else
   asm("createpolicy.fractional.L2::evict_last.b64 %0, 1.0;" : "=l"(p));
-#endif
-  return p;
-}
-__device__ __forceinline__ u64 pol_evict_first() {
-  u64 p;
-#ifdef RSP_EMUL
-  p = 0;
-#else
-  asm("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
 #endif
   return p;
 }
@@ -324,243 +339,29 @@ __device__ __forceinline__ uint4 ldg_pol(const uint4* p, u64 pol) {
 #endif
   return v;
 }
-__device__ __forceinline__ void stg_pol(uint4* p, const uint4& v, u64 pol) {
-#ifdef RSP_EMUL
-  (void)pol;
-  *p = v;
-#else
-  asm volatile("st.global.L2::cache_hint.v4.u32 [%0], {%1,%2,%3,%4}, %5;"
-               :: "l"(p), "r"(v.x), "r"(v.y), "r"(v.z), "r"(v.w), "l"(pol) : "memory");
-#endif
-}
-#ifndef RSP_MG_TPB
-#define RSP_MG_TPB 64
-#endif
-// 20 blocks of 64 threads per SM leave 48 registers per thread.  At 24 blocks (40 registers) ptxas for sm_90a spills
-// k_multi_get16<false> to local memory (60 bytes per thread), and the launch of 8.4 M lookups takes 1.04 ms instead of
-// 0.91 ms on an H100 80GB HBM3 at a 400 W power limit: the spill traffic costs more than the extra lookups in flight buy.
-#ifndef RSP_MG_MINB
-#define RSP_MG_MINB 20
-#endif
 
-// Candidate entry at `ent`: header unit 0, key unit KU, value units KU+1.. (U units in all).
+// Candidate entry at `ent`: header unit 0, key unit KU, value units KU+1.. (U units in all).  CG: a memtable entry
+// (read through L2, its size known only from its header), otherwise a run entry.
 // Returns 0 = served, 1 = not my key (tag false positive), 2 = needs the generic path.
-#ifndef RSP_MG_NOALLOC
-#define RSP_MG_NOALLOC 0  // L1::no_allocate on the entry units (an experiment switch)
-#endif
-#ifndef RSP_MG_MEMSET
-#define RSP_MG_MEMSET 1
-#endif
-__device__ __forceinline__ uint4 ldg_noalloc(const uint4* p) {
-  uint4 v;
-#ifdef RSP_EMUL
-  v = *p;
-#else
-  asm("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "l"(p));
-#endif
-  return v;
-}
 template <bool CG>
-__device__ __forceinline__ uint4 ld_entry_unit(const uint4* p, u64 pol) {
+__device__ __forceinline__ uint4 ld_entry_unit(const uint4* p) {
   if (CG) return __ldcg(p);
-#if RSP_MG_HINTS >= 2
-  return ldg_pol(p, pol);
-#elif RSP_MG_NOALLOC
-  return ldg_noalloc(p);
-#else
   return __ldg(p);
-#endif
 }
 template <bool CG, bool BIG>
 __device__ __forceinline__ u32 fast_entry(const u8* ent, u32 U, u32 KU, const uint4& kq, u64 snap, u8* dst,
-                                          u64 val_stride, u32 lane, u32& vlen_out, u64 pol) {
-  const uint4* ep = reinterpret_cast<const uint4*>(ent);
-  const uint4 hd = ld_entry_unit<CG>(ep, pol);
-  const uint4 ek = ld_entry_unit<CG>(ep + KU, pol);
-  const u32 fv = KU + 1;  // first value unit; lane L owns value units L, L+2, L+4, ...
-  uint4 v0 = make_uint4(0, 0, 0, 0), v1 = v0, v2 = v0;
-  if (!CG) {
-    // a run: the entry size U is known before the header arrives, so the first six value units are
-    // requested together with header and key (one round trip for values up to 96 bytes)
-    if (fv + lane < U) v0 = ld_entry_unit<CG>(ep + fv + lane, pol);
-    if (fv + lane + 2 < U) v1 = ld_entry_unit<CG>(ep + fv + lane + 2, pol);
-    if (fv + lane + 4 < U) v2 = ld_entry_unit<CG>(ep + fv + lane + 4, pol);
-  }
-  if (ek.x != kq.x || ek.y != kq.y || ek.z != kq.z || ek.w != kq.w || hd.z != 16) return 1;
-  const u64 seq = (((u64)hd.y << 32) | hd.x) >> 8;
-  const u32 vu = (hd.w + 15u) >> 4;
-  if ((hd.x & 0xffu) != kTypeValue || seq > snap || (!CG && fv + vu > U) || (u64)vu * 16u > val_stride || (!BIG && vu > 6)) return 2;
-  uint4* out = reinterpret_cast<uint4*>(dst);
-  if (CG) {
-    // the memtable: the entry's size is only known from its header, so the value follows in a second trip
-    for (u32 u = lane; u < vu; u += FL) out[u] = ld_entry_unit<CG>(ep + fv + u, pol);
-  } else {
-#if RSP_MG_HINTS >= 2
-    if (lane < vu) stg_pol(out + lane, v0, pol);
-    if (lane + 2 < vu) stg_pol(out + lane + 2, v1, pol);
-    if (lane + 4 < vu) stg_pol(out + lane + 4, v2, pol);
-#else
-    if (lane < vu) out[lane] = v0;
-    if (lane + 2 < vu) out[lane + 2] = v1;
-    if (lane + 4 < vu) out[lane + 4] = v2;
-#endif
-    if (BIG)
-      for (u32 u = lane + 6; u < vu; u += FL) out[u] = ld_entry_unit<CG>(ep + fv + u, pol);  // values > 96 bytes
-  }
-  vlen_out = hd.w;
-  return 0;
-}
-
-// BIG = false: values up to 96 bytes (larger ones take the pending list); BIG = true adds the tail loop for
-// larger values at the price of a few registers — the host picks by the caller's value stride.
-template <bool BIG>
-__global__ void __launch_bounds__(RSP_MG_TPB, RSP_MG_MINB) k_multi_get16(GetArgs a) {
-  const u32 q = (blockIdx.x * blockDim.x + threadIdx.x) / FL;
-  const u32 lane = threadIdx.x & (FL - 1);
-  const u32 pbase = (threadIdx.x & 31u) & ~1u;
-  const u32 pmask = 3u << pbase;  // the two lanes of this lookup always branch together
-  if (q >= a.n) return;
-  // (1)
-  const u64 pol_stream = pol_evict_first();
-  u32 six = __ldg(a.shard_ix + q);
-  const bool bad_shard = six >= a.max_shards;
-  if (bad_shard) six = 0;
-#if RSP_MG_HINTS >= 2
-  const uint4 kq = ldg_pol(reinterpret_cast<const uint4*>(a.keys) + q, pol_stream);
-#else
-  const uint4 kq = __ldg(reinterpret_cast<const uint4*>(a.keys) + q);
-#endif
-  const uint4 f0 = __ldg(reinterpret_cast<const uint4*>(a.fast + six));
-  const uint4 f1 = __ldg(reinterpret_cast<const uint4*>(a.fast + six) + 1);
-  const u32 n_buckets = f1.x, ord_bits = f1.y & 0xffu, U = (f1.y >> 8) & 0xffu, n_runs = (f1.y >> 16) & 0xffu;
-  const u64 k0 = ((u64)kq.y << 32) | kq.x, k1 = ((u64)kq.w << 32) | kq.z;
-  const u64 h = hash_final(hash_step(hash_step(hash_init(16), k0), k1));
-  u8* dst = a.vals + (u64)q * a.val_stride;
-  u32 state = 3;  // 0 served, 2 generic path, 3 undecided, 4 not found
-  u32 vlen = 0;
-  if (n_runs > 1 || ((a.val_stride | reinterpret_cast<uintptr_t>(a.vals)) & 15u) || bad_shard || !(f1.y >> 24)) state = 2;
-  bool in_mem = false;
-  if (state == 3 && f1.z /* mt_count */) {
-    // the shard's memtable filter (L2-resident, behind the descriptors): a clear bit = the key is not in the memtable
-    const u32 fb = mt_filter_bit(h);
-    const u32 fw = __ldcg(reinterpret_cast<const u32*>(a.fast + (size_t)a.max_shards * (1u + RSP_MAX_RUNS)) + (size_t)six * MT_FILTER_WORDS + (fb >> 5));
-    in_mem = (fw >> (fb & 31u)) & 1u;
-  }
-  if (in_mem) {
-    // ---- memtable: eight u64 slots from the home position, four per lane; descriptor through L2
-    const uint4* dp = reinterpret_cast<const uint4*>(a.shards + six);
-    const uint4 d0 = __ldcg(dp), d1 = __ldcg(dp + 1), d3 = __ldcg(dp + 3);
-    const u8* heap = reinterpret_cast<const u8*>(((u64)d0.y << 32) | d0.x);
-    const u64* sp = reinterpret_cast<const u64*>(((u64)d0.w << 32) | d0.z);
-    const u32 mask = d1.z;
-    const u64 snap = ((u64)d3.w << 32) | d3.z;
-    const u32 tag = hash_tag32(h);
-    u32 cand = 0, info = 0;  // info: matches | (position of my first empty + 1) << 8
-#pragma unroll
-    for (u32 i = 0; i < 4; i++) {
-      const u64 sv = ldcg64(sp + (((u32)h + 4u * lane + i) & mask));
-      if (sv == 0) { if (!(info >> 8)) info |= (4u * lane + i + 1u) << 8; }
-      else if ((u32)(sv >> 32) == tag && !(info >> 8)) { if (!cand) cand = (u32)sv; info++; }
-    }
-    const u32 o_cand = __shfl_xor_sync(pmask, cand, 1), o_info = __shfl_xor_sync(pmask, info, 1);
-    // lane 1's slots come after lane 0's in probe order: they count only if lane 0 saw no empty slot
-    const u32 lo_info = lane ? o_info : info, hi_info = lane ? info : o_info;
-    const u32 lo_cand = lane ? o_cand : cand, hi_cand = lane ? cand : o_cand;
-    const bool lo_empty = (lo_info >> 8) != 0;
-    const u32 n_match = (lo_info & 0xffu) + (lo_empty ? 0u : (hi_info & 0xffu));
-    const bool any_empty = lo_empty || (hi_info >> 8) != 0;
-    if (n_match == 1) {
-      const u32 c = (lo_info & 0xffu) ? lo_cand : hi_cand;
-      // memtable entry: unit0 header, unit1 link, unit2 key, units 3.. value
-      const u32 r = fast_entry<true, BIG>(heap + (u64)(c - 1u) * 16u, 7, 2, kq, snap, dst, a.val_stride, lane, vlen, pol_stream);
-      state = r == 0 ? 0 : 2;
-    } else if (n_match > 1 || !any_empty) {
-      state = 2;
-    }
-  }
-  if (state == 3) {
-    if (n_runs == 0) state = 4;
-    else if (U == 0 || U >= 255) state = 2;
-    else {
-      // ---- run 0 through its hash index: one bucket = one 32-byte sector, four slots per lane
-      const u8* heap = reinterpret_cast<const u8*>(((u64)f0.y << 32) | f0.x);
-      const uint4* hs = reinterpret_cast<const uint4*>(((u64)f0.w << 32) | f0.z);
-      u32 bucket = (u32)(((u64)(u32)h * n_buckets) >> 32);
-      const u32 tag = (u32)(h >> 32) >> ord_bits;
-      // Walk the tag matches in probe order; a false positive (18-bit tags at 16 K entries: ~1 per 60 K
-      // lookups) just moves on to the next candidate, a full bucket to the next bucket.
-      u32 m8 = 0, e8 = 1, probe = 0;  // e8 != 0 before the first load only so that the loop loads first
-      uint4 sv = make_uint4(0, 0, 0, 0);
-      state = 2;
-#pragma unroll 1
-      for (;;) {
-        if (!m8) {
-          if (probe && e8) { state = 4; break; }  // an empty slot ends the probe: NOT_FOUND
-          if (probe == n_buckets) { state = 4; break; }  // (a table without an empty slot)
-          if (probe) bucket = bucket + 1 == n_buckets ? 0 : bucket + 1;
-          probe++;
-#if RSP_MG_HINTS >= 1
-          sv = ldg_pol(hs + (u64)bucket * 2u + lane, pol_evict_last());
-#else
-          sv = __ldg(hs + (u64)bucket * 2u + lane);
-#endif
-          const u32 m = ((sv.x && (sv.x >> ord_bits) == tag) ? 1u : 0u) | ((sv.y && (sv.y >> ord_bits) == tag) ? 2u : 0u) |
-                        ((sv.z && (sv.z >> ord_bits) == tag) ? 4u : 0u) | ((sv.w && (sv.w >> ord_bits) == tag) ? 8u : 0u);
-          const u32 e = (sv.x == 0 || sv.y == 0 || sv.z == 0 || sv.w == 0) ? 1u : 0u;
-          const u32 mine = m | (e << 4);
-          const u32 other = __shfl_xor_sync(pmask, mine, 1);
-          m8 = lane ? ((other & 15u) | ((mine & 15u) << 4)) : ((mine & 15u) | ((other & 15u) << 4));
-          e8 = (mine | other) >> 4;
-          if (!m8) continue;
-        }
-        const u32 p = __ffs(m8) - 1;
-        m8 &= m8 - 1;
-        const u32 pick = (p & 2u) ? ((p & 1u) ? sv.w : sv.z) : ((p & 1u) ? sv.y : sv.x);
-        const u32 val = __shfl_sync(pmask, pick, pbase + (p >> 2));
-        // run entry: unit0 header, unit1 key, units 2.. value
-        const u32 r = fast_entry<false, BIG>(heap + (u64)((val & ((1u << ord_bits) - 1u)) - 1u) * U * 16u, U, 1, kq, ~0ull, dst,
-                                        a.val_stride, lane, vlen, pol_stream);
-        if (r == 0) { state = 0; break; }
-        if (r == 2) break;
-      }
-    }
-  }
-  if (lane == 0) {
-    if (state == 2) {
-      a.pending[atomicAdd(a.n_pending + a.parity, 1u)] = q;
-    } else {
-      a.st[q] = state == 0 ? 0 : 1;
-      a.vlen[q] = vlen;
-    }
-  }
-  // this launch counts in n_pending[parity].  Clearing the other counter here instead of a memset node
-  // before the launch was slower end to end, so the memset node stays (RSP_MG_MEMSET=1).
-#if !RSP_MG_MEMSET
-  if (blockIdx.x == 0 && threadIdx.x == 0) a.n_pending[a.parity ^ 1u] = 0;
-#endif
-}
-
-// Candidate entry at `ent`: header unit 0, key unit KU, value units KU+1.. (U units in all).
-// Returns 0 = served, 1 = not my key (tag false positive), 2 = needs the generic path.
-template <bool CG>
-__device__ __forceinline__ uint4 ld_entry_unit_m(const uint4* p) {
-  if (CG) return __ldcg(p);
-  return __ldg(p);
-}
-template <bool CG, bool BIG>
-__device__ __forceinline__ u32 fast_entry_m(const u8* ent, u32 U, u32 KU, const uint4& kq, u64 snap, u8* dst,
                                           u64 val_stride, u32 lane, u32& vlen_out) {
   const uint4* ep = reinterpret_cast<const uint4*>(ent);
-  const uint4 hd = ld_entry_unit_m<CG>(ep);
-  const uint4 ek = ld_entry_unit_m<CG>(ep + KU);
+  const uint4 hd = ld_entry_unit<CG>(ep);
+  const uint4 ek = ld_entry_unit<CG>(ep + KU);
   const u32 fv = KU + 1;  // first value unit; lane L owns value units L, L+2, L+4, ...
   uint4 v0 = make_uint4(0, 0, 0, 0), v1 = v0, v2 = v0;
   if (!CG) {
     // a run: the entry size U is known before the header arrives, so the first six value units are
     // requested together with header and key (one round trip for values up to 96 bytes)
-    if (fv + lane < U) v0 = ld_entry_unit_m<CG>(ep + fv + lane);
-    if (fv + lane + 2 < U) v1 = ld_entry_unit_m<CG>(ep + fv + lane + 2);
-    if (fv + lane + 4 < U) v2 = ld_entry_unit_m<CG>(ep + fv + lane + 4);
+    if (fv + lane < U) v0 = ld_entry_unit<CG>(ep + fv + lane);
+    if (fv + lane + 2 < U) v1 = ld_entry_unit<CG>(ep + fv + lane + 2);
+    if (fv + lane + 4 < U) v2 = ld_entry_unit<CG>(ep + fv + lane + 4);
   }
   if (ek.x != kq.x || ek.y != kq.y || ek.z != kq.z || ek.w != kq.w || hd.z != 16) return 1;
   const u64 seq = (((u64)hd.y << 32) | hd.x) >> 8;
@@ -569,13 +370,13 @@ __device__ __forceinline__ u32 fast_entry_m(const u8* ent, u32 U, u32 KU, const 
   uint4* out = reinterpret_cast<uint4*>(dst);
   if (CG) {
     // the memtable: the entry's size is only known from its header, so the value follows in a second trip
-    for (u32 u = lane; u < vu; u += FL) out[u] = ld_entry_unit_m<CG>(ep + fv + u);
+    for (u32 u = lane; u < vu; u += FL) out[u] = ld_entry_unit<CG>(ep + fv + u);
   } else {
     if (lane < vu) out[lane] = v0;
     if (lane + 2 < vu) out[lane + 2] = v1;
     if (lane + 4 < vu) out[lane + 4] = v2;
     if (BIG)
-      for (u32 u = lane + 6; u < vu; u += FL) out[u] = ld_entry_unit_m<CG>(ep + fv + u);  // values > 96 bytes
+      for (u32 u = lane + 6; u < vu; u += FL) out[u] = ld_entry_unit<CG>(ep + fv + u);  // values > 96 bytes
   }
   vlen_out = hd.w;
   return 0;
@@ -589,7 +390,7 @@ template <bool BIG>
 __device__ __forceinline__ u32 probe_one_run(const uint4& g0, const uint4& g1, const uint4& kq, u64 h, u8* dst, u64 val_stride,
                                              u32 lane, u32 pmask, u32 pbase, u32& vlen) {
   const u8* heap = reinterpret_cast<const u8*>(((u64)g0.y << 32) | g0.x);
-  const u32 n_buckets = g1.x, ord_bits = g1.y & 0xffu, U = (g1.y >> 8) & 0xffu;
+  const u32 n_buckets = g1.x, ord_bits = g1.y & 0xffu, U = (g1.y >> FAST_META_UNITS_SHIFT) & 0xffu;
   if (U == 0 || U >= 255) return 2;
   const uint4* hs = reinterpret_cast<const uint4*>(((u64)g0.w << 32) | g0.z);
   u32 bucket = (u32)(((u64)(u32)h * n_buckets) >> 32);
@@ -618,20 +419,22 @@ __device__ __forceinline__ u32 probe_one_run(const uint4& g0, const uint4& g1, c
     const u32 pick = (p & 2u) ? ((p & 1u) ? sv.w : sv.z) : ((p & 1u) ? sv.y : sv.x);
     const u32 val = __shfl_sync(pmask, pick, pbase + (p >> 2));
     // run entry: unit0 header, unit1 key, units 2.. value
-    const u32 r = fast_entry_m<false, BIG>(heap + (u64)((val & ((1u << ord_bits) - 1u)) - 1u) * U * 16u, U, 1, kq, ~0ull, dst,
+    const u32 r = fast_entry<false, BIG>(heap + (u64)((val & ((1u << ord_bits) - 1u)) - 1u) * U * 16u, U, 1, kq, ~0ull, dst,
                                          val_stride, lane, vlen);
     if (r == 0) return 0;
     if (r == 2) return 2;
   }
 }
 
-// k_multi_get16m: the same lookup for engines where some shard has SEVERAL sorted runs (between a flush and the next
-// merge): the runs are walked newest first, a run that does not hold the key hands over to the next older one
-// (per-run descriptors behind the ShardFast array).  The single-run kernel above is kept on its own: folding both into
-// one template changes its register allocation at the same instruction mix, so the host picks the kernel per launch.
-template <bool BIG>
-__global__ void __launch_bounds__(RSP_MG_TPB, RSP_MG_MINB) k_multi_get16m(GetArgs a) {
-  constexpr bool MULTI = true;
+// One lookup of the 16-byte-key kernels.  MULTI = false (k_multi_get16): a shard with several sorted runs takes the
+// pending list.  MULTI = true (k_multi_get16m, for engines where some shard has several runs, between a flush and the
+// next merge): the runs are walked newest first, a run that does not hold the key hands over to the next older one
+// (per-run descriptors behind the ShardFast array).  The two stay separate kernels and the host picks one per launch:
+// one kernel with a runtime choice between them changes k_multi_get16's register allocation at the same instruction mix.
+// BIG = false: values up to 96 bytes (larger ones take the pending list); BIG = true adds the tail loop for
+// larger values at the price of a few registers — the host picks by the caller's value stride.
+template <bool BIG, bool MULTI>
+__device__ __forceinline__ void multi_get16(GetArgs a) {
   const u32 q = (blockIdx.x * blockDim.x + threadIdx.x) / FL;
   const u32 lane = threadIdx.x & (FL - 1);
   const u32 pbase = (threadIdx.x & 31u) & ~1u;
@@ -644,7 +447,7 @@ __global__ void __launch_bounds__(RSP_MG_TPB, RSP_MG_MINB) k_multi_get16m(GetArg
   const uint4 kq = __ldg(reinterpret_cast<const uint4*>(a.keys) + q);
   const uint4 f0 = __ldg(reinterpret_cast<const uint4*>(a.fast + six));
   const uint4 f1 = __ldg(reinterpret_cast<const uint4*>(a.fast + six) + 1);
-  const u32 n_runs = (f1.y >> 16) & 0xffu;
+  const u32 n_runs = (f1.y >> FAST_META_RUNS_SHIFT) & 0xffu;
   const u64 k0 = ((u64)kq.y << 32) | kq.x, k1 = ((u64)kq.w << 32) | kq.z;
   const u64 h = hash_final(hash_step(hash_step(hash_init(16), k0), k1));
   u8* dst = a.vals + (u64)q * a.val_stride;
@@ -659,7 +462,7 @@ __global__ void __launch_bounds__(RSP_MG_TPB, RSP_MG_MINB) k_multi_get16m(GetArg
     in_mem = (fw >> (fb & 31u)) & 1u;
   }
   if (in_mem) {
-    // ---- memtable: eight u64 slots from the home position, four per lane; descriptor through L2
+    // ---- (2) memtable: eight u64 slots from the home position, four per lane; descriptor through L2
     const uint4* dp = reinterpret_cast<const uint4*>(a.shards + six);
     const uint4 d0 = __ldcg(dp), d1 = __ldcg(dp + 1), d3 = __ldcg(dp + 3);
     const u8* heap = reinterpret_cast<const u8*>(((u64)d0.y << 32) | d0.x);
@@ -684,17 +487,16 @@ __global__ void __launch_bounds__(RSP_MG_TPB, RSP_MG_MINB) k_multi_get16m(GetArg
     if (n_match == 1) {
       const u32 c = (lo_info & 0xffu) ? lo_cand : hi_cand;
       // memtable entry: unit0 header, unit1 link, unit2 key, units 3.. value
-      const u32 r = fast_entry_m<true, BIG>(heap + (u64)(c - 1u) * 16u, 7, 2, kq, snap, dst, a.val_stride, lane, vlen);
+      const u32 r = fast_entry<true, BIG>(heap + (u64)(c - 1u) * 16u, 7, 2, kq, snap, dst, a.val_stride, lane, vlen);
       state = r == 0 ? 0 : 2;
     } else if (n_match > 1 || !any_empty) {
       state = 2;
     }
   }
   if (state == 3) {
-    // ---- the sorted runs, newest first
+    // (2), (3): the sorted runs, newest first
     state = 4;
-    const u32 nr = MULTI ? n_runs : min(n_runs, 1u);
-    for (u32 r = 0; r < nr; r++) {
+    for (u32 r = 0; r < n_runs; r++) {
       uint4 g0 = f0, g1 = f1;
       if (MULTI && r) {
         const uint4* fr = reinterpret_cast<const uint4*>(a.fast + a.max_shards) + ((u64)six * RSP_MAX_RUNS + r) * 2u;
@@ -702,7 +504,7 @@ __global__ void __launch_bounds__(RSP_MG_TPB, RSP_MG_MINB) k_multi_get16m(GetArg
         g1 = __ldg(fr + 1);
       }
       const u32 rs = probe_one_run<BIG>(g0, g1, kq, h, dst, a.val_stride, lane, pmask, pbase, vlen);
-      if (rs != 4) { state = rs; break; }
+      if (rs != 4 || !MULTI) { state = rs; break; }
     }
   }
   if (lane == 0) {
@@ -714,6 +516,11 @@ __global__ void __launch_bounds__(RSP_MG_TPB, RSP_MG_MINB) k_multi_get16m(GetArg
     }
   }
 }
+
+template <bool BIG>
+__global__ void __launch_bounds__(MG16_THREADS, MG16_MIN_BLOCKS) k_multi_get16(GetArgs a) { multi_get16<BIG, false>(a); }
+template <bool BIG>
+__global__ void __launch_bounds__(MG16_THREADS, MG16_MIN_BLOCKS) k_multi_get16m(GetArgs a) { multi_get16<BIG, true>(a); }
 
 // generic path over the queries the fast kernel deferred; a small fixed grid strides over the list
 __global__ void __launch_bounds__(256) k_multi_get_pending(GetArgs a) {
@@ -731,16 +538,15 @@ bool launch_multi_get(const GetArgs& a, cudaStream_t s) {
   const u32 per_block = 256 / MG_LANES;
   const u32 grid = (a.n + per_block - 1) / per_block;
   if (a.klen_fixed == 16 && (reinterpret_cast<uintptr_t>(a.keys) & 15u) == 0 && a.pending && a.fast) {
-    // this launch counts in n_pending[parity]; a memset node clears it
-#if RSP_MG_MEMSET
+    // this launch counts in n_pending[parity]; a memset node clears it (clearing the other parity's counter inside
+    // the kernel instead is slower end to end)
     cudaMemsetAsync(a.n_pending + a.parity, 0, 4, s);
-#endif
-    const u32 g16 = (a.n + RSP_MG_TPB / FL - 1) / (RSP_MG_TPB / FL);
+    const u32 g16 = (a.n + MG16_THREADS / FL - 1) / (MG16_THREADS / FL);
     const bool multi = a.multirun != 0;
     if (a.val_stride > 96) {
-      if (multi) k_multi_get16m<true><<<g16, RSP_MG_TPB, 0, s>>>(a); else k_multi_get16<true><<<g16, RSP_MG_TPB, 0, s>>>(a);
+      if (multi) k_multi_get16m<true><<<g16, MG16_THREADS, 0, s>>>(a); else k_multi_get16<true><<<g16, MG16_THREADS, 0, s>>>(a);
     } else {
-      if (multi) k_multi_get16m<false><<<g16, RSP_MG_TPB, 0, s>>>(a); else k_multi_get16<false><<<g16, RSP_MG_TPB, 0, s>>>(a);
+      if (multi) k_multi_get16m<false><<<g16, MG16_THREADS, 0, s>>>(a); else k_multi_get16<false><<<g16, MG16_THREADS, 0, s>>>(a);
     }
     k_multi_get_pending<<<std::min<u32>(grid, DEVICE_SMS), 256, 0, s>>>(a);
     return true;
@@ -779,14 +585,12 @@ __global__ void k_get_versions(VersionsArgs a) {
   const u64 o = a.koff[q];
   const u32 klen = (u32)(a.koff[q + 1] - o);
   DumpVisitor v{a.out + (u64)q * a.out_stride, a.out_stride, 0, 0, false};
-  bool stopped;
   if (a.views) {  // a pinned iterator snapshot: sorted runs only
     const ScanView& vw = a.views[q];
     const u64 h = hash_key(a.keys + o, klen);
-    for (u32 ri = 0; ri < vw.n_runs && !v.done; ri++)
-      walk_run<1>(vw.runs[ri], a.keys + o, klen, h, 0, 1u << lane_in_warp, lane_in_warp, v);
+    walk_runs<1>(vw.runs, vw.n_runs, a.keys + o, klen, h, 0, 1u << lane_in_warp, lane_in_warp, v);
   } else {
-    walk_shard<1>(sd, a.keys + o, klen, 0, 1u << lane_in_warp, lane_in_warp, v, stopped);
+    walk_shard<1>(sd, a.keys + o, klen, 0, 1u << lane_in_warp, lane_in_warp, v);
   }
   a.n_rec[q] = v.n_rec;
   a.need[q] = v.used;
@@ -807,56 +611,16 @@ __global__ void __launch_bounds__(256) k_multi_get_at(GetAtArgs a) {
   const u32 gmask = ((1u << MG_LANES) - 1u) << gbase;
   if (q >= a.n) return;
   const u32 slot = __ldg(a.slot + q);
-  if (slot >= a.n_views || !a.views[slot].live) {  // null, released or foreign snapshot
-    if (lane == 0) {
-      a.st[q] = 4;
-      a.vlen[q] = 0;
-      if (a.n_special) atomicAdd(a.n_special, 1u);
-    }
-    return;
-  }
+  if (slot >= a.n_views || !a.views[slot].live) return answer_invalid(a, q, lane);
   const ScanView& vw = a.views[slot];
-  const u8* kp;
   u32 klen;
-  if (a.klen_fixed) {
-    klen = a.klen_fixed;
-    kp = a.keys + (u64)q * klen;
-  } else {
-    const u64 o = __ldg(a.koff + q);
-    klen = (u32)(__ldg(a.koff + q + 1) - o);
-    kp = a.keys + o;
-  }
+  const u8* kp = lookup_key(a, q, klen);
   Acc acc;
   acc.init(vw.merge_op);
   const u64 h = hash_key(kp, klen);
   const u32 n_runs = vw.n_runs;
-  for (u32 ri = 0; ri < n_runs && !acc.done; ri++) walk_run<MG_LANES>(vw.runs[ri], kp, klen, h, lane, gmask, gbase, acc);
-  acc.end_of_versions();
-  i32 st = acc.status;
-  u32 vlen = 0;
-  if (st == 0) {
-    vlen = acc.res_len;
-    if ((u64)vlen > a.val_stride) {
-      st = 7;  // RSP_INCOMPLETE: vlen reports the size needed
-    } else {
-      u8* dst = a.vals + (u64)q * a.val_stride;
-      if (acc.imm) {
-        if (lane == 0) {
-#pragma unroll
-          for (u32 b = 0; b < 8; b++) dst[b] = (u8)(acc.res_imm >> (8u * b));
-        }
-      } else {
-        group_copy_out(dst, acc.res_ptr, vlen, lane, MG_LANES);
-      }
-    }
-  } else if (st != 1 && st != ST_NEED_HOST_MERGE) {
-    vlen = acc.msg;  // message id rides in vlen for error statuses
-  }
-  if (lane == 0) {
-    a.st[q] = st;
-    a.vlen[q] = vlen;
-    if (st != 0 && st != 1 && st != 7 && a.n_special) atomicAdd(a.n_special, 1u);
-  }
+  walk_runs<MG_LANES>(vw.runs, n_runs, kp, klen, h, lane, gmask, gbase, acc);
+  answer(a, q, lane, acc);
 }
 
 void launch_multi_get_at(const GetAtArgs& a, cudaStream_t s) {

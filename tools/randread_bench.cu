@@ -4,9 +4,10 @@
 // dep=0 nothing is serialised: the ceiling k_multi_get16 could approach with enough lookups in flight.  With dep=1
 // the entry address depends on the index sector, as in the engine's probe.
 // idx_mb = 0 skips the index read: one random access per lookup, what an always-L2-resident index would approach.
-// hints = 1 loads like k_multi_get16 does: the index sector with an L2::evict_last policy, the entry units with
-// L2::evict_first (DESIGN §4 has how much of the index that keeps in L2).  The L2 fetch granularity is set to the
-// engine's 32 bytes (RSP_L2_FETCH_BYTES), so every random access is its own sector transaction.
+// hints = 1 loads the index sector with an L2::evict_last policy, as k_multi_get16 does, and the entry units with
+// L2::evict_first, where k_multi_get16 uses plain loads (DESIGN §4 has how much of the index that keeps in L2).
+// The L2 fetch granularity is set to the engine's 32 bytes (RSP_L2_FETCH_BYTES), so every random access is its own
+// sector transaction.
 // The default n is one bench.py MultiGet launch (8.4 M lookups).
 // persist_mb > 0 sets aside that much L2 for persisting (evict_last) lines for this process
 // (cudaLimitPersistingL2CacheSize, capped at the device's persistingL2CacheMaxSize); the engine sets none.
