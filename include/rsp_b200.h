@@ -200,6 +200,14 @@ int rsp_iter_valid(const rsp_iter* it);
 const uint8_t* rsp_iter_key(const rsp_iter* it, size_t* klen);
 const uint8_t* rsp_iter_value(const rsp_iter* it, size_t* vlen);
 int rsp_iter_status(const rsp_iter* it);
+/* ReadOptions::iterate_upper_bound (exclusive, bytewise): the bound is copied; key == NULL clears it.  It applies from
+ * the next positioning call on, to iterators from rsp_iter_create and rsp_iter_create_at alike, and follows RocksDB
+ * 5.4's DBIter: Seek, SeekToFirst and Next stop before the first key >= bound, without walking or merging what lies
+ * beyond it (a failing merge there raises no status); SeekToLast is SeekForPrev(bound) followed by Prev when that
+ * lands on the bound itself; SeekForPrev and Prev do not apply the bound. */
+int rsp_iter_set_upper_bound(rsp_iter* it, const uint8_t* key, size_t klen);
+/* Iterator::SeekForPrev: the last live key <= key */
+void rsp_iter_seek_for_prev(rsp_iter* it, const uint8_t* key, size_t klen);
 
 /* ---- snapshots: DB::GetSnapshot / ReleaseSnapshot and reads with ReadOptions::snapshot ----------------------------
  * A snapshot pins the shard's contents at creation: the memtable's contents are sorted into a private run, and that
@@ -242,6 +250,12 @@ rsp_iter* rsp_iter_create_at(rsp_snapshot* snap);
 int rsp_multi_scan(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys,
                    const uint64_t* koff, uint32_t max_entries, uint8_t* out, size_t out_stride,
                    uint32_t* n_out, int32_t* st);
+/* rsp_multi_scan with an exclusive end key per scan: scan i returns the live entries in [start_i, end_i), up to
+ * max_entries, where end key i is ends[eoff[i] .. eoff[i+1]).  ends == NULL: no scan has an end.  Keys at or beyond the
+ * end are not read: deleted keys and merges there cost nothing and a failing merge there sets no status. */
+int rsp_multi_scan_bounded(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys,
+                           const uint64_t* koff, const uint8_t* ends, const uint64_t* eoff, uint32_t max_entries,
+                           uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st);
 
 /* ---- maintenance: DB::Flush / ApplicationDB::CompactRange(nullptr, nullptr)
  * (application_db.cpp:138-144; triggers admin_handler.cpp:1846,2174) -------------------------------- */
@@ -274,6 +288,11 @@ int rsp_multi_get_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, co
 int rsp_multi_scan_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys,
                           uint32_t klen, uint32_t max_entries, uint8_t* d_out, uint64_t out_stride,
                           uint32_t* d_n_out, int32_t* d_st, void* stream);
+/* rsp_multi_scan_device with an exclusive end key per scan: d_ends[i*end_klen .. +end_klen) (d_ends == NULL: none) */
+int rsp_multi_scan_bounded_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys,
+                                  uint32_t klen, const uint8_t* d_ends, uint32_t end_klen, uint32_t max_entries,
+                                  uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st,
+                                  void* stream);
 /* One apply tick from a pre-staged device image (see rsp_stage_*): decode + sequence + insert.
  * Memtable capacity must have been reserved with rsp_reserve. */
 typedef struct rsp_staged rsp_staged;

@@ -68,11 +68,12 @@ HOST_SRCS = ["gpu_db.cpp", "rocksdb_replicator/rocksdb_replicator.cpp", "rocksdb
 HOST_SO = os.path.join(HERE, "librsp_host.so")
 HOST_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "host_tests")
 SNAPSHOT_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "snapshot_tests")
+BOUNDED_ITER_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "bounded_iter_tests")
 
 
 def build_host(force=False, verbose=False):
-    """The C++ mirror of the reference interfaces (host/) -> librsp_host.so, and its test binaries (the second one,
-    snapshot_tests, is returned by build_snapshot_tests)."""
+    """The C++ mirror of the reference interfaces (host/) -> librsp_host.so, and its test binaries (snapshot_tests and
+    bounded_iter_tests are returned by build_snapshot_tests and build_bounded_iter_tests)."""
     build(force=False, verbose=verbose)
     srcs = [os.path.join(HOST, s) for s in HOST_SRCS]
     deps = list(srcs)
@@ -92,10 +93,10 @@ def build_host(force=False, verbose=False):
     if force or _stale(HOST_TESTS, [tsrc, HOST_SO] + deps):
         run([cxx] + flags + ["-o", HOST_TESTS, tsrc, "-L", HERE, "-lrsp_host", "-lrsp_b200",
                              "-Wl,-rpath," + HERE])
-    ssrc = os.path.join(os.path.dirname(HERE), "tests", "cpp", "snapshot_tests.cpp")
-    if force or _stale(SNAPSHOT_TESTS, [ssrc, HOST_SO] + deps):
-        run([cxx] + flags + ["-o", SNAPSHOT_TESTS, ssrc, "-L", HERE, "-lrsp_host", "-lrsp_b200",
-                             "-Wl,-rpath," + HERE])
+    for exe in (SNAPSHOT_TESTS, BOUNDED_ITER_TESTS):
+        src = exe + ".cpp"
+        if force or _stale(exe, [src, HOST_SO] + deps):
+            run([cxx] + flags + ["-o", exe, src, "-L", HERE, "-lrsp_host", "-lrsp_b200", "-Wl,-rpath," + HERE])
     return HOST_SO, HOST_TESTS
 
 
@@ -103,3 +104,10 @@ def build_snapshot_tests(force=False, verbose=False):
     """tests/cpp/snapshot_tests: GpuDB / ApplicationDB reads with ReadOptions::snapshot"""
     build_host(force=force, verbose=verbose)
     return SNAPSHOT_TESTS
+
+
+def build_bounded_iter_tests(force=False, verbose=False):
+    """tests/cpp/bounded_iter_tests: GpuDB / ApplicationDB iterators with ReadOptions::iterate_upper_bound and
+    SeekForPrev"""
+    build_host(force=force, verbose=verbose)
+    return BOUNDED_ITER_TESTS

@@ -1543,6 +1543,8 @@ struct rsp_iter {
   int status = 0;
   size_t want = 16;
   size_t stride = 16384;
+  bool has_upper = false;    // ReadOptions::iterate_upper_bound (exclusive): forward fetches end there
+  std::string upper;
 };
 
 // DBIter's status_ is sticky and is raised when the iterator REACHES a key whose merge fails (it keeps that key, with
@@ -1560,11 +1562,13 @@ static void iter_fetch(rsp_iter* it, const std::string* key, bool exclusive, boo
   it->pos = 0;
   it->reverse = reverse;
   std::string fetch_key;
+  const bool bounded = it->has_upper && !reverse;
+  const size_t elen = bounded ? it->upper.size() : 0;
   for (;;) {
     const size_t klen = key ? key->size() : 0;
-    const size_t o_key = 64, o_out = 64 + align_up(klen + 16, 256);
+    const size_t o_key = 64, o_ekey = 64 + align_up(klen + 16, 256), o_out = o_ekey + align_up(elen + 16, 256);
     u8* d = (u8*)e->dev_q.get(o_out + it->stride + 256);
-    // header: [koff 2x8][flags 1][pad][n_out 4 @32][st 4 @36]
+    // header: [koff 2x8][flags 1][pad][n_out 4 @32][st 4 @36][pad][eoff 2x8 @40]
     u64 koff[2] = {0, klen};
     u8 flags = (exclusive ? 1 : 0) | (reverse ? 2 : 0) | (key ? 0 : 4);
     CUDA_OK(cudaMemcpyAsync(d, koff, 16, cudaMemcpyHostToDevice, e->st));
@@ -1574,6 +1578,12 @@ static void iter_fetch(rsp_iter* it, const std::string* key, bool exclusive, boo
     a.shards = nullptr; a.views = it->d_view; a.shard_ix = nullptr; a.keys = d + o_key; a.koff = (const u64*)d;
     a.klen_fixed = 0; a.flags = d + 16; a.max_entries = (u32)it->want; a.out = d + o_out; a.out_stride = it->stride;
     a.n_out = (u32*)(d + 32); a.st = (i32*)(d + 36); a.n = 1;
+    if (bounded) {
+      const u64 eoff[2] = {0, elen};
+      CUDA_OK(cudaMemcpyAsync(d + 40, eoff, 16, cudaMemcpyHostToDevice, e->st));
+      if (elen) CUDA_OK(cudaMemcpyAsync(d + o_ekey, it->upper.data(), elen, cudaMemcpyHostToDevice, e->st));
+      a.ends = d + o_ekey; a.eoff = (const u64*)(d + 40);
+    }
     launch_multi_scan(a, e->st);
     e->launches++;
     u32 res[2];
@@ -2779,8 +2789,28 @@ void rsp_iter_seek_to_first(rsp_iter* it) {
 }
 void rsp_iter_seek_to_last(rsp_iter* it) {
   try {
-    it->want = 16; iter_fetch(it, nullptr, false, true);
+    it->want = 16;
+    if (!it->has_upper) { iter_fetch(it, nullptr, false, true); return; }
+    // DBIter (RocksDB 5.4) under an upper bound: SeekForPrev(bound), then Prev when it landed on the bound itself
+    const std::string k = it->upper;
+    iter_fetch(it, &k, false, true);
+    if (it->valid && it->buf[it->pos].first == k) rsp_iter_prev(it);
   } catch (...) { abi_caught(); it->valid = false; it->status = RSP_IO_ERROR; }
+}
+void rsp_iter_seek_for_prev(rsp_iter* it, const uint8_t* key, size_t klen) {
+  try {
+  std::string k((const char*)key, klen);
+  it->want = 16;
+  iter_fetch(it, &k, false, true);  // the last live key <= key; RocksDB 5.4 applies no upper bound here
+  } catch (...) { abi_caught(); }
+}
+int rsp_iter_set_upper_bound(rsp_iter* it, const uint8_t* key, size_t klen) {
+  if (!it) return RSP_INVALID_ARGUMENT;
+  try {
+  it->has_upper = key != nullptr;
+  it->upper.assign(key ? (const char*)key : "", key ? klen : 0);
+  return RSP_OK;
+  } catch (...) { return abi_caught(); }
 }
 void rsp_iter_seek(rsp_iter* it, const uint8_t* key, size_t klen) {
   try {
@@ -2974,10 +3004,11 @@ int rsp_multi_get_at_device(rsp_engine* e, size_t n, const uint32_t* d_slot, con
 }
 
 // ---- batched scans (host buffers) ----
-int rsp_multi_scan(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
-                   uint32_t max_entries, uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st) {
-  try {
-  if (!e || (n && (!shard_ix || !koff || !out || !n_out || !st))) return RSP_INVALID_ARGUMENT;
+// rsp_multi_scan / rsp_multi_scan_bounded (ends == nullptr: no end keys)
+static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
+                           const uint8_t* ends, const uint64_t* eoff, uint32_t max_entries, uint8_t* out,
+                           size_t out_stride, uint32_t* n_out, int32_t* st) {
+  if (!e || (n && (!shard_ix || !koff || !out || !n_out || !st || (ends && !eoff)))) return RSP_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(e->mu);
   CUDA_OK(cudaSetDevice(e->device));
   if (n == 0) return RSP_OK;
@@ -2989,9 +3020,10 @@ int rsp_multi_scan(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint
     if (s->h.mt_count && std::find(fl.begin(), fl.end(), s) == fl.end()) fl.push_back(s);
   }
   if (!fl.empty()) compact_shards(e, fl, false);
-  const size_t key_bytes = (size_t)koff[n];
+  const size_t key_bytes = (size_t)koff[n], end_bytes = ends ? (size_t)eoff[n] : 0;
   const size_t o_koff = align_up(n * 4, 256), o_keys = o_koff + align_up((n + 1) * 8, 256);
-  const size_t o_nout = o_keys + align_up(key_bytes + 16, 256), o_st = o_nout + align_up(n * 4, 256);
+  const size_t o_eoff = o_keys + align_up(key_bytes + 16, 256), o_ends = o_eoff + (ends ? align_up((n + 1) * 8, 256) : 0);
+  const size_t o_nout = o_ends + (ends ? align_up(end_bytes + 16, 256) : 0), o_st = o_nout + align_up(n * 4, 256);
   const size_t o_out = o_st + align_up(n * 4, 256);
   u8* d = (u8*)e->dev_q.get(o_out + n * out_stride + 256);
   CUDA_OK(cudaMemcpyAsync(d, shard_ix, n * 4, cudaMemcpyHostToDevice, e->st));
@@ -3001,6 +3033,11 @@ int rsp_multi_scan(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint
   a.shards = e->d_shards; a.views = nullptr; a.shard_ix = (const u32*)d; a.keys = d + o_keys;
   a.koff = (const u64*)(d + o_koff); a.klen_fixed = 0; a.flags = nullptr; a.max_entries = max_entries;
   a.out = d + o_out; a.out_stride = out_stride; a.n_out = (u32*)(d + o_nout); a.st = (i32*)(d + o_st); a.n = (u32)n;
+  if (ends) {
+    CUDA_OK(cudaMemcpyAsync(d + o_eoff, eoff, (n + 1) * 8, cudaMemcpyHostToDevice, e->st));
+    if (end_bytes) CUDA_OK(cudaMemcpyAsync(d + o_ends, ends, end_bytes, cudaMemcpyHostToDevice, e->st));
+    a.ends = d + o_ends; a.eoff = (const u64*)(d + o_eoff);
+  }
   CUDA_OK(cudaEventRecord(e->ev0, e->st));
   launch_multi_scan(a, e->st);
   e->launches++;
@@ -3029,6 +3066,18 @@ int rsp_multi_scan(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint
     }
   }
   return RSP_OK;
+}
+int rsp_multi_scan(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
+                   uint32_t max_entries, uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st) {
+  try {
+    return multi_scan_host(e, n, shard_ix, keys, koff, nullptr, nullptr, max_entries, out, out_stride, n_out, st);
+  } catch (...) { return abi_caught(); }
+}
+int rsp_multi_scan_bounded(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
+                           const uint8_t* ends, const uint64_t* eoff, uint32_t max_entries, uint8_t* out,
+                           size_t out_stride, uint32_t* n_out, int32_t* st) {
+  try {
+    return multi_scan_host(e, n, shard_ix, keys, koff, ends, eoff, max_entries, out, out_stride, n_out, st);
   } catch (...) { return abi_caught(); }
 }
 
@@ -3056,15 +3105,16 @@ int rsp_multi_get_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, co
   } catch (...) { return abi_caught(); }
 }
 
-int rsp_multi_scan_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys, uint32_t klen,
-                          uint32_t max_entries, uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st,
-                          void* stream) {
-  try {
+// rsp_multi_scan_device / rsp_multi_scan_bounded_device (d_ends == nullptr: no end keys)
+static int multi_scan_dev(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys, uint32_t klen,
+                          const uint8_t* d_ends, uint32_t end_klen, uint32_t max_entries, uint8_t* d_out,
+                          uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st, void* stream) {
   if (!e || !klen) return RSP_INVALID_ARGUMENT;
   ScanArgs a;
   a.shards = e->d_shards; a.views = nullptr; a.shard_ix = d_shard_ix; a.keys = d_keys; a.koff = nullptr;
   a.klen_fixed = klen; a.flags = nullptr; a.max_entries = max_entries; a.out = d_out; a.out_stride = out_stride;
   a.n_out = d_n_out; a.st = d_st; a.n = (u32)n;
+  a.ends = d_ends; a.elen = end_klen;
   {
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t rs = stream ? (cudaStream_t)stream : e->st;
@@ -3074,6 +3124,21 @@ int rsp_multi_scan_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, c
   }
   e->launches++;
   return cudaPeekAtLastError() == cudaSuccess ? RSP_OK : RSP_IO_ERROR;
+}
+int rsp_multi_scan_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys, uint32_t klen,
+                          uint32_t max_entries, uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st,
+                          void* stream) {
+  try {
+    return multi_scan_dev(e, n, d_shard_ix, d_keys, klen, nullptr, 0, max_entries, d_out, out_stride, d_n_out, d_st,
+                          stream);
+  } catch (...) { return abi_caught(); }
+}
+int rsp_multi_scan_bounded_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys,
+                                  uint32_t klen, const uint8_t* d_ends, uint32_t end_klen, uint32_t max_entries,
+                                  uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st, void* stream) {
+  try {
+    return multi_scan_dev(e, n, d_shard_ix, d_keys, klen, d_ends, end_klen, max_entries, d_out, out_stride, d_n_out,
+                          d_st, stream);
   } catch (...) { return abi_caught(); }
 }
 

@@ -737,13 +737,15 @@ __device__ __forceinline__ bool mbar_wait(u64* mbar, u32 parity) {
 }
 #endif
 
-// warp-cooperative lower bound: first ordinal of R whose key is >= key (strict: > key)
-__device__ u32 run_lower_bound_warp(const RunDev& R, const u8* kp, u32 klen, bool strict, u64* s_pfx, u64* mbar,
+// warp-cooperative lower bound: first ordinal of R whose key is >= key (strict: > key).  mbar: R's block index is being
+// copied into s_pfx by the bulk copy that completes the mbarrier's phase 0 (issued once per scan; later searches find
+// the phase complete); nullptr: a run of several blocks is searched in global memory.
+__device__ u32 run_lower_bound_warp(const RunDev& R, const u8* kp, u32 klen, bool strict, const u64* s_pfx, u64* mbar,
                                     u32 lane) {
   u32 lo = 0, hi = R.n_ent;
   if (R.n_blocks > 1 && klen) {
-    if (lane == 0) tma_load_1d(s_pfx, R.blk_pfx, (R.n_blocks * 8u + 15u) & ~15u, mbar);
-    const u64 pfx = key_prefix_be(kp, klen);
+    if (!mbar) return run_lower_bound(R, kp, klen, strict);
+    const u64 pfx = key_prefix_be(kp, klen);  // (the key's load overlaps the bulk copy)
     if (!__all_sync(0xffffffffu, mbar_wait(mbar, 0))) return run_lower_bound(R, kp, klen, strict);
     u32 n_lt = 0, n_le = 0;
     for (u32 b = 0; b < R.n_blocks; b += 32) {
@@ -770,6 +772,8 @@ __device__ u32 run_lower_bound_warp(const RunDev& R, const u8* kp, u32 klen, boo
   return lo + below;
 }
 
+// BOUNDED: the requests carry end keys (a.ends); the unbounded instance has none of the end-key code
+template <bool BOUNDED>
 __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
   __shared__ __align__(16) u64 s_pfx_all[SCAN_WARPS][SCAN_STAGE_PFX];
   __shared__ __align__(8) u64 s_mbar[SCAN_WARPS];
@@ -795,6 +799,14 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
   else { const u64 o = a.koff[q]; klen = (u32)(a.koff[q + 1] - o); kp = a.keys + o; }
   const u32 fl = a.flags ? a.flags[q] : 0u;
   const bool exclusive = fl & 1u, reverse = fl & 2u, extreme = fl & 4u;
+  // the end key (exclusive; forward scans stop there)
+  const bool has_end = BOUNDED && !reverse;
+  const u8* ekp = nullptr;
+  u32 eklen = 0;
+  if (has_end) {
+    if (a.eoff) { const u64 o = a.eoff[q]; eklen = (u32)(a.eoff[q + 1] - o); ekp = a.ends + o; }
+    else { eklen = a.elen; ekp = a.ends + (u64)q * eklen; }
+  }
   u8* out = a.out + (u64)q * a.out_stride;
   u64 used = 0;
   u32 n_out = 0;
@@ -808,13 +820,20 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
     const u32 kl = R.kv_len & 0xffffu, vl = R.kv_len >> 16;
     const u32 rec = 8u + kl + vl;
     if ((kl & 15u) == 0 && (vl & 7u) == 0 && ((reinterpret_cast<uintptr_t>(out) | a.out_stride) & 7u) == 0) {
-      u32 start = 0;
-      if (!extreme) {
-        const u32 wi = threadIdx.x >> 5;
-        start = R.n_blocks <= SCAN_STAGE_PFX ? run_lower_bound_warp(R, kp, klen, exclusive, s_pfx_all[wi], &s_mbar[wi], lane)
-                                             : run_lower_bound(R, kp, klen, exclusive);
+      // ONE bulk copy of the block index (when a search needs it) serves the start and the end search
+      const u32 wi = threadIdx.x >> 5;
+      u64* mbar = nullptr;
+      if (R.n_blocks > 1 && R.n_blocks <= SCAN_STAGE_PFX && ((!extreme && klen) || (has_end && eklen))) {
+        mbar = &s_mbar[wi];
+        if (lane == 0) tma_load_1d(s_pfx_all[wi], R.blk_pfx, (R.n_blocks * 8u + 15u) & ~15u, mbar);
       }
+      const u64* s_pfx = s_pfx_all[wi];
+      const u32 start = extreme ? 0u : run_lower_bound_warp(R, kp, klen, exclusive, s_pfx, mbar, lane);
       u32 cnt = min(a.max_entries, R.n_ent - start);
+      if (has_end) {
+        const u32 end = run_lower_bound_warp(R, ekp, eklen, false, s_pfx, mbar, lane);
+        cnt = end > start ? min(cnt, end - start) : 0u;
+      }
       i32 fst = 0;
       if ((u64)cnt * rec > a.out_stride) { cnt = (u32)(a.out_stride / rec); fst = 7; }
       const u32 wpr = rec >> 3;  // 8-byte words per record
@@ -911,6 +930,12 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
       bk.e = reinterpret_cast<const u8*>(__shfl_sync(0xffffffffu, (u64)reinterpret_cast<uintptr_t>(h_e), w));
       bk.klen = __shfl_sync(0xffffffffu, h_klen, w);
       bk.vlen = 0; bk.type = 0;
+      // the end key: checked before any version is visited, so that deleted keys, merge operands and host-folded keys
+      // at or beyond it are never walked, folded or reported
+      if (has_end) {
+        const u64 epfx = key_prefix_be(ekp, eklen);
+        if (mp > epfx || (mp == epfx && cmp_key_vs_padded(ekp, eklen, bk.key(), bk.klen) <= 0)) break;
+      }
       // newest run first; inside a run the versions of a key follow each other, newest first
       for (u32 g = group; g;) {
         const u32 r = (u32)__ffs(g) - 1u;
@@ -999,10 +1024,12 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
   }
 }
 
-__global__ void __launch_bounds__(128) k_multi_scan(ScanArgs a) { multi_scan_body(a); }
+template <bool BOUNDED>
+__global__ void __launch_bounds__(128) k_multi_scan(ScanArgs a) { multi_scan_body<BOUNDED>(a); }
 
 void launch_multi_scan(const ScanArgs& a, cudaStream_t s) {
   if (!a.n) return;
-  k_multi_scan<<<(a.n + 3) / 4, 128, 0, s>>>(a);
+  if (a.ends) k_multi_scan<true><<<(a.n + 3) / 4, 128, 0, s>>>(a);
+  else k_multi_scan<false><<<(a.n + 3) / 4, 128, 0, s>>>(a);
 }
 }  // namespace rsp

@@ -196,6 +196,11 @@ struct ScanArgs {
   u32* n_out;
   i32* st;
   u32 n;
+  // optional exclusive end key per request, forward scans only: ends[eoff[q] .. eoff[q+1]), or ends + q * elen when
+  // eoff == nullptr.  ends == nullptr: no end.
+  const u8* ends = nullptr;
+  const u64* eoff = nullptr;
+  u32 elen = 0;
 };
 void launch_multi_scan(const ScanArgs& a, cudaStream_t s);
 

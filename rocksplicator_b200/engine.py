@@ -83,6 +83,8 @@ EXPORTS = {
     "rsp_iter_key": (C.c_void_p, [C.c_void_p, C.POINTER(C.c_size_t)]),
     "rsp_iter_value": (C.c_void_p, [C.c_void_p, C.POINTER(C.c_size_t)]),
     "rsp_iter_status": (C.c_int, [C.c_void_p]),
+    "rsp_iter_set_upper_bound": (C.c_int, [C.c_void_p, C.c_char_p, C.c_size_t]),
+    "rsp_iter_seek_for_prev": (None, [C.c_void_p, C.c_char_p, C.c_size_t]),
     "rsp_snapshot_create": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p)]),
     "rsp_snapshot_release": (None, [C.c_void_p]),
     "rsp_snapshot_seq": (C.c_uint64, [C.c_void_p]),
@@ -95,6 +97,8 @@ EXPORTS = {
     "rsp_iter_create_at": (C.c_void_p, [C.c_void_p]),
     "rsp_multi_scan": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
                                  C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    "rsp_multi_scan_bounded": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     "rsp_flush": (C.c_int, [C.c_void_p]),
     "rsp_compact": (C.c_int, [C.c_void_p]),
     "rsp_flush_all": (C.c_int, [C.c_void_p]),
@@ -106,6 +110,9 @@ EXPORTS = {
                                        C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rsp_multi_scan_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32,
                                         C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "rsp_multi_scan_bounded_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
+                                                C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
+                                                C.c_void_p]),
     "rsp_stage_build": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.POINTER(C.c_void_p)]),
     "rsp_stage_free": (None, [C.c_void_p]),
@@ -145,10 +152,19 @@ def _ptr(a):
 
 
 class Iterator:
-    def __init__(self, shard, snapshot=None):
+    """upper_bound: ReadOptions::iterate_upper_bound (exclusive; None = no bound)"""
+
+    def __init__(self, shard, snapshot=None, upper_bound=None):
         self.lib = shard.lib
         self.h = self.lib.rsp_iter_create(shard.h) if snapshot is None else self.lib.rsp_iter_create_at(snapshot.h)
         self._shard = shard
+        if upper_bound is not None:
+            self.set_upper_bound(upper_bound)
+
+    def set_upper_bound(self, key):
+        rc = self.lib.rsp_iter_set_upper_bound(self.h, key, 0 if key is None else len(key))
+        if rc != OK:
+            raise RuntimeError(f"rsp_iter_set_upper_bound -> {rc}")
 
     def close(self):
         if self.h:
@@ -164,6 +180,7 @@ class Iterator:
     def seek_to_first(self): self.lib.rsp_iter_seek_to_first(self.h)
     def seek_to_last(self): self.lib.rsp_iter_seek_to_last(self.h)
     def seek(self, k): self.lib.rsp_iter_seek(self.h, k, len(k))
+    def seek_for_prev(self, k): self.lib.rsp_iter_seek_for_prev(self.h, k, len(k))
     def next(self): self.lib.rsp_iter_next(self.h)
     def prev(self): self.lib.rsp_iter_prev(self.h)
     def valid(self): return bool(self.lib.rsp_iter_valid(self.h))
@@ -219,11 +236,12 @@ class Snapshot:
     def multi_get(self, keys, stride=256):
         return self.shard.engine.multi_get_at([self] * len(keys), keys, stride)
 
-    def iterator(self):
-        return Iterator(self.shard, self)
+    def iterator(self, upper_bound=None):
+        return Iterator(self.shard, self, upper_bound)
 
-    def scan(self, start=None, limit=None):
-        it = self.iterator()
+    def scan(self, start=None, limit=None, end=None):
+        """up to `limit` live entries from `start` (None: the first key) to `end` (exclusive; None: the last key)"""
+        it = self.iterator(upper_bound=end)
         if start is None:
             it.seek_to_first()
         else:
@@ -291,14 +309,15 @@ class Shard:
         res = self.engine.multi_get([self.index] * len(keys), keys, stride)
         return res
 
-    def iterator(self):
-        return Iterator(self)
+    def iterator(self, upper_bound=None):
+        return Iterator(self, upper_bound=upper_bound)
 
     def snapshot(self):
         return Snapshot(self)
 
-    def scan(self, start=None, limit=None):
-        it = self.iterator()
+    def scan(self, start=None, limit=None, end=None):
+        """up to `limit` live entries from `start` (None: the first key) to `end` (exclusive; None: the last key)"""
+        it = self.iterator(upper_bound=end)
         if start is None:
             it.seek_to_first()
         else:
@@ -427,7 +446,9 @@ class Engine:
         return self.lib.rsp_multi_get_fixed(self.h, len(six), _ptr(six), _ptr(keys), klen, _ptr(vals), stride,
                                             _ptr(vlen), _ptr(st))
 
-    def multi_scan(self, shard_ix, keys, max_entries, stride):
+    def multi_scan(self, shard_ix, keys, max_entries, stride, ends=None):
+        """scan i: up to max_entries live entries from keys[i], before ends[i] (exclusive) when ends is given ->
+        [(status, [(key, value)])]"""
         n = len(keys)
         six = np.ascontiguousarray(shard_ix, dtype=np.uint32)
         off = np.zeros(n + 1, dtype=np.uint64)
@@ -436,8 +457,17 @@ class Engine:
         out = np.zeros(max(n * stride, 1), dtype=np.uint8)
         n_out = np.zeros(max(n, 1), dtype=np.uint32)
         st = np.zeros(max(n, 1), dtype=np.int32)
-        rc = self.lib.rsp_multi_scan(self.h, n, _ptr(six), _ptr(blob), _ptr(off), max_entries, _ptr(out), stride,
-                                     _ptr(n_out), _ptr(st))
+        if ends is None:
+            rc = self.lib.rsp_multi_scan(self.h, n, _ptr(six), _ptr(blob), _ptr(off), max_entries, _ptr(out), stride,
+                                         _ptr(n_out), _ptr(st))
+        else:
+            if len(ends) != n:
+                raise ValueError("one end key per scan")
+            eoff = np.zeros(n + 1, dtype=np.uint64)
+            np.cumsum(np.fromiter((len(k) for k in ends), dtype=np.uint64, count=n), out=eoff[1:])
+            eblob = np.frombuffer(b"".join(ends) + b"\0", dtype=np.uint8)
+            rc = self.lib.rsp_multi_scan_bounded(self.h, n, _ptr(six), _ptr(blob), _ptr(off), _ptr(eblob), _ptr(eoff),
+                                                 max_entries, _ptr(out), stride, _ptr(n_out), _ptr(st))
         if rc != OK:
             raise RuntimeError(f"rsp_multi_scan -> {rc}")
         res = []

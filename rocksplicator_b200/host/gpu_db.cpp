@@ -528,6 +528,7 @@ class GpuIterator : public rocksdb::Iterator {
   void SeekToFirst() override { rsp_iter_seek_to_first(it_); }
   void SeekToLast() override { rsp_iter_seek_to_last(it_); }
   void Seek(const Slice& t) override { rsp_iter_seek(it_, (const uint8_t*)t.data(), t.size()); }
+  void SeekForPrev(const Slice& t) override { rsp_iter_seek_for_prev(it_, (const uint8_t*)t.data(), t.size()); }
   void Next() override { rsp_iter_next(it_); }
   void Prev() override { rsp_iter_prev(it_); }
   Slice key() const override { size_t n; auto p = rsp_iter_key(it_, &n); return Slice((const char*)p, n); }
@@ -543,7 +544,10 @@ class GpuIterator : public rocksdb::Iterator {
 }  // namespace
 
 rocksdb::Iterator* GpuDB::NewIterator(const rocksdb::ReadOptions& o) {
-  return new GpuIterator(o.snapshot ? rsp_iter_create_at(RawSnapshot(o.snapshot)) : rsp_iter_create(shard_));
+  rsp_iter* it = o.snapshot ? rsp_iter_create_at(RawSnapshot(o.snapshot)) : rsp_iter_create(shard_);
+  if (it && o.iterate_upper_bound)  // the engine keeps its own copy of the bound
+    rsp_iter_set_upper_bound(it, (const uint8_t*)o.iterate_upper_bound->data(), o.iterate_upper_bound->size());
+  return new GpuIterator(it);
 }
 
 Status GpuDB::CompactRange(const rocksdb::CompactRangeOptions&, const Slice* begin, const Slice* end) {

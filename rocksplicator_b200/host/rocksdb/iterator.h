@@ -12,6 +12,8 @@ class Iterator {
   virtual void SeekToFirst() = 0;
   virtual void SeekToLast() = 0;
   virtual void Seek(const Slice& target) = 0;
+  // positions at the last key <= target
+  virtual void SeekForPrev(const Slice& target) = 0;
   virtual void Next() = 0;
   virtual void Prev() = 0;
   virtual Slice key() const = 0;

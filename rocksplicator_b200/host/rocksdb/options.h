@@ -8,9 +8,16 @@
 namespace rocksdb {
 class MergeOperator;
 class Snapshot;
+class Slice;
 struct WriteOptions { bool sync = false; bool disableWAL = false; };
 // snapshot: read as of DB::GetSnapshot's handle (nullptr = the latest state)
-struct ReadOptions { bool verify_checksums = true; bool fill_cache = true; const Snapshot* snapshot = nullptr; };
+struct ReadOptions {
+  bool verify_checksums = true;
+  bool fill_cache = true;
+  const Snapshot* snapshot = nullptr;
+  // exclusive upper bound of an iterator's forward moves (bytewise); the Slice must outlive the iterator
+  const Slice* iterate_upper_bound = nullptr;
+};
 struct CompactRangeOptions { bool change_level = false; int target_level = -1; };
 struct FlushOptions { bool wait = true; };
 // rocksdb_admin/admin_handler.cpp:1820-1828 sets move_files and allow_global_seqno, the rest stay default
