@@ -256,6 +256,15 @@ int rsp_multi_scan(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint
 int rsp_multi_scan_bounded(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys,
                            const uint64_t* koff, const uint8_t* ends, const uint64_t* eoff, uint32_t max_entries,
                            uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st);
+/* Batched reverse scans: Iterator::SeekForPrev + Prev.  Scan i starts at the last live key <= key i (< key i when
+ * exclusive != 0; keys == NULL: every scan starts at the shard's last key, as SeekToLast, and koff is not read) and
+ * returns up to max_entries live entries in DESCENDING key order.  lows != NULL: scan i stops before the first key
+ * < low i, where low i = lows[loff[i] .. loff[i+1]) is inclusive.  Keys below the low, and with exclusive the start key
+ * itself, are not read.  So [a, b) newest-first is key b, exclusive, low a.  Records, n_out, st and the flush-first
+ * rule are those of rsp_multi_scan. */
+int rsp_multi_scan_reverse(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
+                           int exclusive, const uint8_t* lows, const uint64_t* loff, uint32_t max_entries,
+                           uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st);
 
 /* ---- maintenance: DB::Flush / ApplicationDB::CompactRange(nullptr, nullptr)
  * (application_db.cpp:138-144; triggers admin_handler.cpp:1846,2174) -------------------------------- */
@@ -293,6 +302,13 @@ int rsp_multi_scan_bounded_device(rsp_engine* e, size_t n, const uint32_t* d_sha
                                   uint32_t klen, const uint8_t* d_ends, uint32_t end_klen, uint32_t max_entries,
                                   uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st,
                                   void* stream);
+/* rsp_multi_scan_reverse on device pointers, runs only, as rsp_multi_scan_device: start key i is
+ * d_keys[i*klen .. +klen) (d_keys == NULL: every scan starts at the shard's last key), inclusive low i
+ * d_lows[i*low_klen .. +low_klen) (d_lows == NULL: no low) */
+int rsp_multi_scan_reverse_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys,
+                                  uint32_t klen, int exclusive, const uint8_t* d_lows, uint32_t low_klen,
+                                  uint32_t max_entries, uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out,
+                                  int32_t* d_st, void* stream);
 /* One apply tick from a pre-staged device image (see rsp_stage_*): decode + sequence + insert.
  * Memtable capacity must have been reserved with rsp_reserve. */
 typedef struct rsp_staged rsp_staged;

@@ -1568,15 +1568,14 @@ static void iter_fetch(rsp_iter* it, const std::string* key, bool exclusive, boo
     const size_t klen = key ? key->size() : 0;
     const size_t o_key = 64, o_ekey = 64 + align_up(klen + 16, 256), o_out = o_ekey + align_up(elen + 16, 256);
     u8* d = (u8*)e->dev_q.get(o_out + it->stride + 256);
-    // header: [koff 2x8][flags 1][pad][n_out 4 @32][st 4 @36][pad][eoff 2x8 @40]
+    // header: [koff 2x8][pad][n_out 4 @32][st 4 @36][pad][eoff 2x8 @40]
     u64 koff[2] = {0, klen};
-    u8 flags = (exclusive ? 1 : 0) | (reverse ? 2 : 0) | (key ? 0 : 4);
     CUDA_OK(cudaMemcpyAsync(d, koff, 16, cudaMemcpyHostToDevice, e->st));
-    CUDA_OK(cudaMemcpyAsync(d + 16, &flags, 1, cudaMemcpyHostToDevice, e->st));
     if (klen) CUDA_OK(cudaMemcpyAsync(d + o_key, key->data(), klen, cudaMemcpyHostToDevice, e->st));
     ScanArgs a;
     a.shards = nullptr; a.views = it->d_view; a.shard_ix = nullptr; a.keys = d + o_key; a.koff = (const u64*)d;
-    a.klen_fixed = 0; a.flags = d + 16; a.max_entries = (u32)it->want; a.out = d + o_out; a.out_stride = it->stride;
+    a.klen_fixed = 0; a.flags = (exclusive ? SCAN_EXCLUSIVE : 0u) | (key ? 0u : SCAN_FROM_EXTREME);
+    a.max_entries = (u32)it->want; a.out = d + o_out; a.out_stride = it->stride;
     a.n_out = (u32*)(d + 32); a.st = (i32*)(d + 36); a.n = 1;
     if (bounded) {
       const u64 eoff[2] = {0, elen};
@@ -1584,7 +1583,7 @@ static void iter_fetch(rsp_iter* it, const std::string* key, bool exclusive, boo
       if (elen) CUDA_OK(cudaMemcpyAsync(d + o_ekey, it->upper.data(), elen, cudaMemcpyHostToDevice, e->st));
       a.ends = d + o_ekey; a.eoff = (const u64*)(d + 40);
     }
-    launch_multi_scan(a, e->st);
+    launch_multi_scan(a, reverse, e->st);
     e->launches++;
     u32 res[2];
     CUDA_OK(cudaMemcpyAsync(res, d + 32, 8, cudaMemcpyDeviceToHost, e->st));
@@ -3004,11 +3003,14 @@ int rsp_multi_get_at_device(rsp_engine* e, size_t n, const uint32_t* d_slot, con
 }
 
 // ---- batched scans (host buffers) ----
-// rsp_multi_scan / rsp_multi_scan_bounded (ends == nullptr: no end keys)
+// rsp_multi_scan / rsp_multi_scan_bounded / rsp_multi_scan_reverse (ends == nullptr: no end keys; for reverse scans
+// the ends are the lows, and keys == nullptr starts every scan at the shard's last key)
 static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
-                           const uint8_t* ends, const uint64_t* eoff, uint32_t max_entries, uint8_t* out,
-                           size_t out_stride, uint32_t* n_out, int32_t* st) {
-  if (!e || (n && (!shard_ix || !koff || !out || !n_out || !st || (ends && !eoff)))) return RSP_INVALID_ARGUMENT;
+                           const uint8_t* ends, const uint64_t* eoff, bool reverse, bool exclusive,
+                           uint32_t max_entries, uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st) {
+  const bool from_last = reverse && !keys;
+  if (!e || (n && (!shard_ix || (!koff && !from_last) || !out || !n_out || !st || (ends && !eoff))))
+    return RSP_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(e->mu);
   CUDA_OK(cudaSetDevice(e->device));
   if (n == 0) return RSP_OK;
@@ -3020,6 +3022,8 @@ static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, co
     if (s->h.mt_count && std::find(fl.begin(), fl.end(), s) == fl.end()) fl.push_back(s);
   }
   if (!fl.empty()) compact_shards(e, fl, false);
+  std::vector<uint64_t> no_keys;
+  if (from_last) { no_keys.assign(n + 1, 0); koff = no_keys.data(); }
   const size_t key_bytes = (size_t)koff[n], end_bytes = ends ? (size_t)eoff[n] : 0;
   const size_t o_koff = align_up(n * 4, 256), o_keys = o_koff + align_up((n + 1) * 8, 256);
   const size_t o_eoff = o_keys + align_up(key_bytes + 16, 256), o_ends = o_eoff + (ends ? align_up((n + 1) * 8, 256) : 0);
@@ -3031,7 +3035,8 @@ static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, co
   if (key_bytes) CUDA_OK(cudaMemcpyAsync(d + o_keys, keys, key_bytes, cudaMemcpyHostToDevice, e->st));
   ScanArgs a;
   a.shards = e->d_shards; a.views = nullptr; a.shard_ix = (const u32*)d; a.keys = d + o_keys;
-  a.koff = (const u64*)(d + o_koff); a.klen_fixed = 0; a.flags = nullptr; a.max_entries = max_entries;
+  a.koff = (const u64*)(d + o_koff); a.klen_fixed = 0; a.max_entries = max_entries;
+  a.flags = (exclusive ? SCAN_EXCLUSIVE : 0u) | (from_last ? SCAN_FROM_EXTREME : 0u);
   a.out = d + o_out; a.out_stride = out_stride; a.n_out = (u32*)(d + o_nout); a.st = (i32*)(d + o_st); a.n = (u32)n;
   if (ends) {
     CUDA_OK(cudaMemcpyAsync(d + o_eoff, eoff, (n + 1) * 8, cudaMemcpyHostToDevice, e->st));
@@ -3039,7 +3044,7 @@ static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, co
     a.ends = d + o_ends; a.eoff = (const u64*)(d + o_eoff);
   }
   CUDA_OK(cudaEventRecord(e->ev0, e->st));
-  launch_multi_scan(a, e->st);
+  launch_multi_scan(a, reverse, e->st);
   e->launches++;
   CUDA_OK(cudaEventRecord(e->ev1, e->st));
   CUDA_OK(cudaMemcpyAsync(n_out, d + o_nout, n * 4, cudaMemcpyDeviceToHost, e->st));
@@ -3070,14 +3075,24 @@ static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, co
 int rsp_multi_scan(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
                    uint32_t max_entries, uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st) {
   try {
-    return multi_scan_host(e, n, shard_ix, keys, koff, nullptr, nullptr, max_entries, out, out_stride, n_out, st);
+    return multi_scan_host(e, n, shard_ix, keys, koff, nullptr, nullptr, false, false, max_entries, out, out_stride,
+                           n_out, st);
   } catch (...) { return abi_caught(); }
 }
 int rsp_multi_scan_bounded(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
                            const uint8_t* ends, const uint64_t* eoff, uint32_t max_entries, uint8_t* out,
                            size_t out_stride, uint32_t* n_out, int32_t* st) {
   try {
-    return multi_scan_host(e, n, shard_ix, keys, koff, ends, eoff, max_entries, out, out_stride, n_out, st);
+    return multi_scan_host(e, n, shard_ix, keys, koff, ends, eoff, false, false, max_entries, out, out_stride, n_out,
+                           st);
+  } catch (...) { return abi_caught(); }
+}
+int rsp_multi_scan_reverse(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
+                           int exclusive, const uint8_t* lows, const uint64_t* loff, uint32_t max_entries,
+                           uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st) {
+  try {
+    return multi_scan_host(e, n, shard_ix, keys, koff, lows, loff, true, exclusive != 0, max_entries, out, out_stride,
+                           n_out, st);
   } catch (...) { return abi_caught(); }
 }
 
@@ -3105,21 +3120,25 @@ int rsp_multi_get_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, co
   } catch (...) { return abi_caught(); }
 }
 
-// rsp_multi_scan_device / rsp_multi_scan_bounded_device (d_ends == nullptr: no end keys)
+// rsp_multi_scan_device / rsp_multi_scan_bounded_device / rsp_multi_scan_reverse_device (d_ends == nullptr: no end
+// keys; for reverse scans the ends are the lows, and d_keys == nullptr starts every scan at the shard's last key)
 static int multi_scan_dev(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys, uint32_t klen,
-                          const uint8_t* d_ends, uint32_t end_klen, uint32_t max_entries, uint8_t* d_out,
-                          uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st, void* stream) {
-  if (!e || !klen) return RSP_INVALID_ARGUMENT;
+                          const uint8_t* d_ends, uint32_t end_klen, bool reverse, bool exclusive, uint32_t max_entries,
+                          uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st, void* stream) {
+  const bool from_last = reverse && !d_keys;
+  if (!e || (!klen && !from_last)) return RSP_INVALID_ARGUMENT;
   ScanArgs a;
   a.shards = e->d_shards; a.views = nullptr; a.shard_ix = d_shard_ix; a.keys = d_keys; a.koff = nullptr;
-  a.klen_fixed = klen; a.flags = nullptr; a.max_entries = max_entries; a.out = d_out; a.out_stride = out_stride;
+  a.klen_fixed = from_last ? 1u : klen;  // (from the last key: the keys are not read)
+  a.flags = (exclusive ? SCAN_EXCLUSIVE : 0u) | (from_last ? SCAN_FROM_EXTREME : 0u);
+  a.max_entries = max_entries; a.out = d_out; a.out_stride = out_stride;
   a.n_out = d_n_out; a.st = d_st; a.n = (u32)n;
   a.ends = d_ends; a.elen = end_klen;
   {
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t rs = stream ? (cudaStream_t)stream : e->st;
     reader_begin(e, rs);
-    launch_multi_scan(a, rs);
+    launch_multi_scan(a, reverse, rs);
     reader_end(e, rs);
   }
   e->launches++;
@@ -3129,16 +3148,25 @@ int rsp_multi_scan_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, c
                           uint32_t max_entries, uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st,
                           void* stream) {
   try {
-    return multi_scan_dev(e, n, d_shard_ix, d_keys, klen, nullptr, 0, max_entries, d_out, out_stride, d_n_out, d_st,
-                          stream);
+    return multi_scan_dev(e, n, d_shard_ix, d_keys, klen, nullptr, 0, false, false, max_entries, d_out, out_stride,
+                          d_n_out, d_st, stream);
   } catch (...) { return abi_caught(); }
 }
 int rsp_multi_scan_bounded_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys,
                                   uint32_t klen, const uint8_t* d_ends, uint32_t end_klen, uint32_t max_entries,
                                   uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st, void* stream) {
   try {
-    return multi_scan_dev(e, n, d_shard_ix, d_keys, klen, d_ends, end_klen, max_entries, d_out, out_stride, d_n_out,
-                          d_st, stream);
+    return multi_scan_dev(e, n, d_shard_ix, d_keys, klen, d_ends, end_klen, false, false, max_entries, d_out,
+                          out_stride, d_n_out, d_st, stream);
+  } catch (...) { return abi_caught(); }
+}
+int rsp_multi_scan_reverse_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys,
+                                  uint32_t klen, int exclusive, const uint8_t* d_lows, uint32_t low_klen,
+                                  uint32_t max_entries, uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out,
+                                  int32_t* d_st, void* stream) {
+  try {
+    return multi_scan_dev(e, n, d_shard_ix, d_keys, klen, d_lows, low_klen, true, exclusive != 0, max_entries, d_out,
+                          out_stride, d_n_out, d_st, stream);
   } catch (...) { return abi_caught(); }
 }
 

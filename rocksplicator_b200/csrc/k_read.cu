@@ -772,8 +772,9 @@ __device__ u32 run_lower_bound_warp(const RunDev& R, const u8* kp, u32 klen, boo
   return lo + below;
 }
 
-// BOUNDED: the requests carry end keys (a.ends); the unbounded instance has none of the end-key code
-template <bool BOUNDED>
+// BOUNDED: the requests carry end keys (a.ends; the low, for reverse scans); the unbounded instance has none of the
+// end-key code.  REVERSE: SeekForPrev + Prev (descending keys); the forward instances have none of the reverse code.
+template <bool BOUNDED, bool REVERSE>
 __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
   __shared__ __align__(16) u64 s_pfx_all[SCAN_WARPS][SCAN_STAGE_PFX];
   __shared__ __align__(8) u64 s_mbar[SCAN_WARPS];
@@ -797,10 +798,9 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
   u32 klen;
   if (a.klen_fixed) { klen = a.klen_fixed; kp = a.keys + (u64)q * klen; }
   else { const u64 o = a.koff[q]; klen = (u32)(a.koff[q + 1] - o); kp = a.keys + o; }
-  const u32 fl = a.flags ? a.flags[q] : 0u;
-  const bool exclusive = fl & 1u, reverse = fl & 2u, extreme = fl & 4u;
-  // the end key (exclusive; forward scans stop there)
-  const bool has_end = BOUNDED && !reverse;
+  const bool exclusive = a.flags & SCAN_EXCLUSIVE, extreme = a.flags & SCAN_FROM_EXTREME;
+  // the end key: forward scans stop before it, reverse scans before the first key below it
+  const bool has_end = BOUNDED;
   const u8* ekp = nullptr;
   u32 eklen = 0;
   if (has_end) {
@@ -812,10 +812,10 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
   u32 n_out = 0;
   i32 st = 0;
 
-  // ---- fast path: one fully compacted run of fixed-size Puts, forward scan.  Seek (block index + binary
-  // search), then the warp streams the consecutive entries out as 8-byte words: record i =
-  // [u32 klen][u32 vlen][key][value] at out + i * (8 + klen + vlen).
-  if (n_runs == 1 && !reverse && (runs[0].flags & RUN_ALL_PUT_FIXED)) {
+  // ---- fast path: one fully compacted run of fixed-size Puts.  Seek (block index + binary search), then the warp
+  // streams the consecutive entries out as 8-byte words: record i = [u32 klen][u32 vlen][key][value] at
+  // out + i * (8 + klen + vlen) is entry start + i (forward) or start - i (reverse, start = the last entry <= key).
+  if (n_runs == 1 && (runs[0].flags & RUN_ALL_PUT_FIXED)) {
     const RunDev& R = runs[0];
     const u32 kl = R.kv_len & 0xffffu, vl = R.kv_len >> 16;
     const u32 rec = 8u + kl + vl;
@@ -828,11 +828,20 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
         if (lane == 0) tma_load_1d(s_pfx_all[wi], R.blk_pfx, (R.n_blocks * 8u + 15u) & ~15u, mbar);
       }
       const u64* s_pfx = s_pfx_all[wi];
-      const u32 start = extreme ? 0u : run_lower_bound_warp(R, kp, klen, exclusive, s_pfx, mbar, lane);
-      u32 cnt = min(a.max_entries, R.n_ent - start);
-      if (has_end) {
-        const u32 end = run_lower_bound_warp(R, ekp, eklen, false, s_pfx, mbar, lane);
-        cnt = end > start ? min(cnt, end - start) : 0u;
+      u32 start, cnt;
+      if constexpr (REVERSE) {
+        // entries [lo, p) are <= key (< key when exclusive) and >= the low; they go out from p - 1 down
+        const u32 p = extreme ? R.n_ent : run_lower_bound_warp(R, kp, klen, !exclusive, s_pfx, mbar, lane);
+        const u32 lo = has_end ? run_lower_bound_warp(R, ekp, eklen, false, s_pfx, mbar, lane) : 0u;
+        start = p - 1u;  // (unused when p == 0: cnt is 0)
+        cnt = p > lo ? min(a.max_entries, p - lo) : 0u;
+      } else {
+        start = extreme ? 0u : run_lower_bound_warp(R, kp, klen, exclusive, s_pfx, mbar, lane);
+        cnt = min(a.max_entries, R.n_ent - start);
+        if (has_end) {
+          const u32 end = run_lower_bound_warp(R, ekp, eklen, false, s_pfx, mbar, lane);
+          cnt = end > start ? min(cnt, end - start) : 0u;
+        }
       }
       i32 fst = 0;
       if ((u64)cnt * rec > a.out_stride) { cnt = (u32)(a.out_stride / rec); fst = 7; }
@@ -849,8 +858,9 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
           const u32 w = w0 + 32u * u;
           if (w < total) {
             const u32 r = w / wpr, jw = w - r * wpr;
-            // source words of entry r: word 1 = (klen, vlen); key from word 2; value follows (klen % 16 == 0)
-            v[u] = __ldg(src + (u64)r * R.uniform_units * 2u + 1 + jw);
+            // source words of record r: word 1 = (klen, vlen); key from word 2; value follows (klen % 16 == 0)
+            const u64 off = (u64)r * R.uniform_units * 2u;
+            v[u] = __ldg((REVERSE ? src - off : src + off) + 1 + jw);
           }
         }
 #pragma unroll
@@ -867,75 +877,100 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
     }
   }
 
-  // ---- general path: k-way newest-wins merge over the pinned runs.
-  // FORWARD scans are lane-parallel: lane r owns run r's cursor and keeps its head entry cached (pointer, lengths,
-  // type, 8-byte big-endian key prefix).  Every lane seeks its own run at the same time; per output key the warp takes
-  // the minimum prefix by shuffles, settles prefix ties by full-key compares done in parallel by the tied lanes, and
-  // the runs that hold the key are visited newest first while their lanes already load their next heads.
-  // REVERSE scans (Iterator::Prev, rare) keep the scalar walk: every lane executes the same code.
-  u32 cur[RSP_MAX_RUNS];
-  // forward state of lane r (r < n_runs)
+  // ---- general path: k-way newest-wins merge over the pinned runs, lane-parallel.  Lane r owns run r's cursor and
+  // keeps its head entry cached (pointer, lengths, type, 8-byte big-endian key prefix).  Every lane seeks its own run at
+  // the same time; per output key the warp takes the minimum (reverse: maximum) prefix by shuffles, settles prefix ties
+  // by full-key compares done in parallel by the tied lanes, and the runs that hold the key are visited newest first
+  // while their lanes already load their next heads.  Forward, the head is entry my_cur.  Reverse, it is entry
+  // my_cur - 1 (my_cur = the number of entries <= key, or < key when exclusive), the oldest version of its key.
   u32 my_cur = 0, h_klen = 0, h_vlen = 0, h_type = 0;
   const u8* h_e = nullptr;
   u64 h_pfx = 0;
   bool h_valid = false;
   auto load_head = [&]() {
-    h_valid = lane < n_runs && my_cur < runs[lane].n_ent;
+    h_valid = lane < n_runs && (REVERSE ? my_cur > 0 : my_cur < runs[lane].n_ent);
     if (h_valid) {
-      h_e = run_entry(runs[lane], my_cur);
+      h_e = run_entry(runs[lane], REVERSE ? my_cur - 1u : my_cur);
       const uint4 hd = __ldg(reinterpret_cast<const uint4*>(h_e));
       h_type = hd.x & 0xffu; h_klen = hd.z; h_vlen = hd.w;
       h_pfx = h_klen ? bswap64(__ldg(reinterpret_cast<const u64*>(h_e + 16))) : 0ull;
     }
   };
-  if (!reverse) {
-    if (lane < n_runs) my_cur = extreme ? 0u : run_lower_bound(runs[lane], kp, klen, exclusive);
-    load_head();
-  } else {
-    for (u32 r = 0; r < n_runs; r++) {
-      if (extreme) cur[r] = runs[r].n_ent;
-      else cur[r] = run_lower_bound(runs[r], kp, klen, !exclusive);  // entries < key (or <= key)
-    }
+  if (lane < n_runs) {
+    if constexpr (REVERSE) my_cur = extreme ? runs[lane].n_ent : run_lower_bound(runs[lane], kp, klen, !exclusive);
+    else my_cur = extreme ? 0u : run_lower_bound(runs[lane], kp, klen, exclusive);
   }
+  load_head();
 
   while (n_out < a.max_entries) {
     EntRef bk;
     Acc acc;
     acc.init(merge_op);
-    if (!reverse) {
-      const u32 vmask = __ballot_sync(0xffffffffu, h_valid);
-      if (!vmask) break;
-      // minimum prefix over the valid heads (lanes 0 .. 7 hold the runs: three butterfly steps)
-      u64 mp = h_valid ? h_pfx : ~0ull;
+    const u32 vmask = __ballot_sync(0xffffffffu, h_valid);
+    if (!vmask) break;
+    // minimum (reverse: maximum) prefix over the valid heads (lanes 0 .. 7 hold the runs: three butterfly steps)
+    u64 mp = h_valid ? h_pfx : (REVERSE ? 0ull : ~0ull);
 #pragma unroll
-      for (u32 d = 1; d < RSP_MAX_RUNS; d <<= 1) {
-        const u64 o = __shfl_xor_sync(0xffffffffu, mp, d);
-        mp = o < mp ? o : mp;
-      }
-      mp = __shfl_sync(0xffffffffu, mp, 0);
-      u32 cand = __ballot_sync(0xffffffffu, h_valid && h_pfx == mp);
-      u32 group, w;
-      for (;;) {  // the smallest full key among the tied prefixes, and every run whose head is that key
-        w = (u32)__ffs(cand) - 1u;
-        const u64 wk = __shfl_sync(0xffffffffu, (u64)reinterpret_cast<uintptr_t>(h_e), w);
-        const u32 wkl = __shfl_sync(0xffffffffu, h_klen, w);
-        int c = 0;
-        const bool mine = ((cand >> lane) & 1u) && lane != w;
-        if (mine) c = cmp_padded(reinterpret_cast<const u64*>(h_e + 16), h_klen, reinterpret_cast<const u64*>(reinterpret_cast<const u8*>(wk) + 16), wkl);
-        const u32 less = __ballot_sync(0xffffffffu, mine && c < 0);
-        if (less) { cand = less; continue; }
-        group = __ballot_sync(0xffffffffu, mine && c == 0) | (1u << w);
-        break;
-      }
-      bk.e = reinterpret_cast<const u8*>(__shfl_sync(0xffffffffu, (u64)reinterpret_cast<uintptr_t>(h_e), w));
-      bk.klen = __shfl_sync(0xffffffffu, h_klen, w);
-      bk.vlen = 0; bk.type = 0;
-      // the end key: checked before any version is visited, so that deleted keys, merge operands and host-folded keys
-      // at or beyond it are never walked, folded or reported
-      if (has_end) {
-        const u64 epfx = key_prefix_be(ekp, eklen);
+    for (u32 d = 1; d < RSP_MAX_RUNS; d <<= 1) {
+      const u64 o = __shfl_xor_sync(0xffffffffu, mp, d);
+      mp = (REVERSE ? o > mp : o < mp) ? o : mp;
+    }
+    mp = __shfl_sync(0xffffffffu, mp, 0);
+    u32 cand = __ballot_sync(0xffffffffu, h_valid && h_pfx == mp);
+    u32 group, w;
+    for (;;) {  // the smallest (reverse: largest) full key among the tied prefixes, and every run whose head is that key
+      w = (u32)__ffs(cand) - 1u;
+      const u64 wk = __shfl_sync(0xffffffffu, (u64)reinterpret_cast<uintptr_t>(h_e), w);
+      const u32 wkl = __shfl_sync(0xffffffffu, h_klen, w);
+      int c = 0;
+      const bool mine = ((cand >> lane) & 1u) && lane != w;
+      if (mine) c = cmp_padded(reinterpret_cast<const u64*>(h_e + 16), h_klen, reinterpret_cast<const u64*>(reinterpret_cast<const u8*>(wk) + 16), wkl);
+      const u32 ahead = __ballot_sync(0xffffffffu, mine && (REVERSE ? c > 0 : c < 0));
+      if (ahead) { cand = ahead; continue; }
+      group = __ballot_sync(0xffffffffu, mine && c == 0) | (1u << w);
+      break;
+    }
+    bk.e = reinterpret_cast<const u8*>(__shfl_sync(0xffffffffu, (u64)reinterpret_cast<uintptr_t>(h_e), w));
+    bk.klen = __shfl_sync(0xffffffffu, h_klen, w);
+    bk.vlen = 0; bk.type = 0;
+    // the end key (reverse: the low): checked before any version is visited, so that deleted keys, merge operands and
+    // host-folded keys at or beyond the end (below the low) are never walked, folded or reported
+    if (has_end) {
+      const u64 epfx = key_prefix_be(ekp, eklen);
+      if constexpr (REVERSE) {
+        if (mp < epfx || (mp == epfx && cmp_key_vs_padded(ekp, eklen, bk.key(), bk.klen) > 0)) break;
+      } else {
         if (mp > epfx || (mp == epfx && cmp_key_vs_padded(ekp, eklen, bk.key(), bk.klen) <= 0)) break;
       }
+    }
+    if constexpr (REVERSE) {
+      // the versions of a key lie together in a run, newest first, so the head is the oldest: each run that holds the
+      // key walks down to the group's first (newest) entry, and the entry below it becomes its next head.  The group is
+      // then [my_cur, top); its last entry is the old head, kept in o_e / o_type / o_vlen.
+      const u32 top = my_cur, o_type = h_type, o_vlen = h_vlen;
+      const u8* o_e = h_e;
+      if ((group >> lane) & 1u) {
+        do {
+          my_cur--;
+          load_head();
+        } while (h_valid && h_pfx == mp &&
+                 cmp_padded(reinterpret_cast<const u64*>(h_e + 16), h_klen, bk.key(), bk.klen) == 0);
+      }
+      const u32 voff = 16u + 16u * units_of(bk.klen);
+      // newest run first, newest version first
+      for (u32 g = group; g && !acc.done;) {
+        const u32 r = (u32)__ffs(g) - 1u;
+        g &= g - 1u;
+        const u32 lo = __shfl_sync(0xffffffffu, my_cur, r), hi = __shfl_sync(0xffffffffu, top, r);
+        for (u32 o = lo; o + 1u < hi && !acc.done; o++) {
+          const EntRef x = load_ent(runs[r], o);
+          acc.visit(x.type, x.val(), x.vlen);
+        }
+        const u32 t = __shfl_sync(0xffffffffu, o_type, r), vl = __shfl_sync(0xffffffffu, o_vlen, r);
+        const u64 ep = __shfl_sync(0xffffffffu, (u64)reinterpret_cast<uintptr_t>(o_e), r);
+        if (!acc.done) acc.visit(t, reinterpret_cast<const u8*>(ep) + voff, vl);
+      }
+    } else {
       // newest run first; inside a run the versions of a key follow each other, newest first
       for (u32 g = group; g;) {
         const u32 r = (u32)__ffs(g) - 1u;
@@ -954,33 +989,6 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
           if (!__shfl_sync(0xffffffffu, (u32)same, r)) break;
         }
       }
-    } else {
-    // pick the next user key: the maximum over the reverse cursors (newest run wins ties)
-    int best = -1;
-    for (u32 r = 0; r < n_runs; r++) {
-      if (cur[r] == 0) continue;
-      const EntRef x = load_ent(runs[r], cur[r] - 1);
-      if (best < 0) { best = (int)r; bk = x; continue; }
-      const int c = cmp_padded(x.key(), x.klen, bk.key(), bk.klen);
-      if (c > 0) { best = (int)r; bk = x; }
-    }
-    if (best < 0) break;
-    // resolve this key across the runs that hold it, newest run first
-    for (u32 r = 0; r < n_runs; r++) {
-      const RunDev& R = runs[r];
-      // group = [g, cur[r]) with the same key; versions are newest-first from g upward
-      u32 g = cur[r];
-      while (g > 0) {
-        const EntRef x = load_ent(R, g - 1);
-        if (cmp_padded(x.key(), x.klen, bk.key(), bk.klen) != 0) break;
-        g--;
-      }
-      for (u32 o = g; o < cur[r] && !acc.done; o++) {
-        const EntRef x = load_ent(R, o);
-        acc.visit(x.type, x.val(), x.vlen);
-      }
-      cur[r] = g;
-    }
     }
     acc.end_of_versions();
     if (acc.status == 1) continue;  // deleted
@@ -1024,12 +1032,20 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
   }
 }
 
-template <bool BOUNDED>
-__global__ void __launch_bounds__(128) k_multi_scan(ScanArgs a) { multi_scan_body<BOUNDED>(a); }
+// (a minimum of one block: with __launch_bounds__(128) alone ptxas holds the instances to 64 or 72 registers and spills
+// three of them; with it none spills)
+template <bool BOUNDED, bool REVERSE>
+__global__ void __launch_bounds__(128, 1) k_multi_scan(ScanArgs a) { multi_scan_body<BOUNDED, REVERSE>(a); }
 
-void launch_multi_scan(const ScanArgs& a, cudaStream_t s) {
+void launch_multi_scan(const ScanArgs& a, bool reverse, cudaStream_t s) {
   if (!a.n) return;
-  if (a.ends) k_multi_scan<true><<<(a.n + 3) / 4, 128, 0, s>>>(a);
-  else k_multi_scan<false><<<(a.n + 3) / 4, 128, 0, s>>>(a);
+  const u32 blocks = (a.n + 3) / 4;
+  if (reverse) {
+    if (a.ends) k_multi_scan<true, true><<<blocks, 128, 0, s>>>(a);
+    else k_multi_scan<false, true><<<blocks, 128, 0, s>>>(a);
+  } else {
+    if (a.ends) k_multi_scan<true, false><<<blocks, 128, 0, s>>>(a);
+    else k_multi_scan<false, false><<<blocks, 128, 0, s>>>(a);
+  }
 }
 }  // namespace rsp

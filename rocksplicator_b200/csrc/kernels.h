@@ -189,20 +189,24 @@ struct ScanArgs {
   const u8* keys;
   const u64* koff;
   u32 klen_fixed;
-  const u8* flags;          // per request: bit0 = exclusive start, bit1 = reverse, bit2 = from extreme
+  u32 flags;                // every request: SCAN_EXCLUSIVE, SCAN_FROM_EXTREME
   u32 max_entries;
   u8* out;
   u64 out_stride;
   u32* n_out;
   i32* st;
   u32 n;
-  // optional exclusive end key per request, forward scans only: ends[eoff[q] .. eoff[q+1]), or ends + q * elen when
-  // eoff == nullptr.  ends == nullptr: no end.
+  // optional end key per request in the scan's direction: ends[eoff[q] .. eoff[q+1]), or ends + q * elen when
+  // eoff == nullptr.  ends == nullptr: no end.  Forward scans stop before the end (exclusive); reverse scans stop before
+  // the first key below it (the low is inclusive).
   const u8* ends = nullptr;
   const u64* eoff = nullptr;
   u32 elen = 0;
 };
-void launch_multi_scan(const ScanArgs& a, cudaStream_t s);
+constexpr u32 SCAN_EXCLUSIVE = 1;      // start after the key (forward: > key; reverse: < key)
+constexpr u32 SCAN_FROM_EXTREME = 2;   // ignore the keys: start at the first (forward) or last (reverse) key
+// reverse: Iterator::SeekForPrev + Prev (descending keys); otherwise Seek + Next
+void launch_multi_scan(const ScanArgs& a, bool reverse, cudaStream_t s);
 
 // ---- flush / compaction ---------------------------------------------------------------------------
 struct SortItem {

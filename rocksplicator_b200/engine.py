@@ -99,6 +99,9 @@ EXPORTS = {
                                  C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
     "rsp_multi_scan_bounded": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    "rsp_multi_scan_reverse": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                         C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p,
+                                         C.c_void_p]),
     "rsp_flush": (C.c_int, [C.c_void_p]),
     "rsp_compact": (C.c_int, [C.c_void_p]),
     "rsp_flush_all": (C.c_int, [C.c_void_p]),
@@ -113,6 +116,9 @@ EXPORTS = {
     "rsp_multi_scan_bounded_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
                                                 C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p,
                                                 C.c_void_p]),
+    "rsp_multi_scan_reverse_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int,
+                                                C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p,
+                                                C.c_void_p, C.c_void_p]),
     "rsp_stage_build": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.POINTER(C.c_void_p)]),
     "rsp_stage_free": (None, [C.c_void_p]),
@@ -149,6 +155,33 @@ def load_library():
 
 def _ptr(a):
     return a.ctypes.data_as(C.c_void_p) if a is not None else None
+
+
+def _pack_keys(keys):
+    """byte strings -> (blob, offsets): key i is blob[off[i] .. off[i+1])"""
+    off = np.zeros(len(keys) + 1, dtype=np.uint64)
+    np.cumsum(np.fromiter((len(k) for k in keys), dtype=np.uint64, count=len(keys)), out=off[1:])
+    return np.frombuffer(b"".join(keys) + b"\0", dtype=np.uint8), off
+
+
+def _scan_records(out, n_out, st, n, stride):
+    """the [u32 klen][u32 vlen][key][value] records of n scans at out + i * stride -> [(status, [(key, value)])].  A key
+    that needs the host-side merge operator (vlen 0xffffffff, no value bytes; the scan's status is NotSupported) comes
+    back as (key, None)."""
+    res = []
+    for i in range(n):
+        recs, at = [], i * stride
+        for _ in range(int(n_out[i])):
+            kl = int(out[at:at + 4].view(np.uint32)[0])
+            vl = int(out[at + 4:at + 8].view(np.uint32)[0])
+            if vl == 0xffffffff:
+                recs.append((out[at + 8:at + 8 + kl].tobytes(), None))
+                at += 8 + kl
+                continue
+            recs.append((out[at + 8:at + 8 + kl].tobytes(), out[at + 8 + kl:at + 8 + kl + vl].tobytes()))
+            at += 8 + kl + vl
+        res.append((int(st[i]), recs))
+    return res
 
 
 class Iterator:
@@ -451,9 +484,7 @@ class Engine:
         [(status, [(key, value)])]"""
         n = len(keys)
         six = np.ascontiguousarray(shard_ix, dtype=np.uint32)
-        off = np.zeros(n + 1, dtype=np.uint64)
-        np.cumsum(np.fromiter((len(k) for k in keys), dtype=np.uint64, count=n), out=off[1:])
-        blob = np.frombuffer(b"".join(keys) + b"\0", dtype=np.uint8)
+        blob, off = _pack_keys(keys)
         out = np.zeros(max(n * stride, 1), dtype=np.uint8)
         n_out = np.zeros(max(n, 1), dtype=np.uint32)
         st = np.zeros(max(n, 1), dtype=np.int32)
@@ -463,23 +494,34 @@ class Engine:
         else:
             if len(ends) != n:
                 raise ValueError("one end key per scan")
-            eoff = np.zeros(n + 1, dtype=np.uint64)
-            np.cumsum(np.fromiter((len(k) for k in ends), dtype=np.uint64, count=n), out=eoff[1:])
-            eblob = np.frombuffer(b"".join(ends) + b"\0", dtype=np.uint8)
+            eblob, eoff = _pack_keys(ends)
             rc = self.lib.rsp_multi_scan_bounded(self.h, n, _ptr(six), _ptr(blob), _ptr(off), _ptr(eblob), _ptr(eoff),
                                                  max_entries, _ptr(out), stride, _ptr(n_out), _ptr(st))
         if rc != OK:
             raise RuntimeError(f"rsp_multi_scan -> {rc}")
-        res = []
-        for i in range(n):
-            recs, at = [], i * stride
-            for _ in range(int(n_out[i])):
-                kl = int(out[at:at + 4].view(np.uint32)[0])
-                vl = int(out[at + 4:at + 8].view(np.uint32)[0])
-                recs.append((out[at + 8:at + 8 + kl].tobytes(), out[at + 8 + kl:at + 8 + kl + vl].tobytes()))
-                at += 8 + kl + vl
-            res.append((int(st[i]), recs))
-        return res
+        return _scan_records(out, n_out, st, n, stride)
+
+    def multi_scan_reverse(self, shard_ix, keys, max_entries, stride, lows=None, exclusive=False):
+        """reverse scan i (SeekForPrev + Prev): up to max_entries live entries in descending key order from the last key
+        <= keys[i] (< keys[i] when exclusive; keys=None: from the shard's last key), down to lows[i] (inclusive) when
+        lows is given -> [(status, [(key, value)])].  [a, b) newest-first: keys=[b], lows=[a], exclusive=True."""
+        n = len(shard_ix)
+        six = np.ascontiguousarray(shard_ix, dtype=np.uint32)
+        if keys is not None and len(keys) != n:
+            raise ValueError("one start key per scan")
+        if lows is not None and len(lows) != n:
+            raise ValueError("one low key per scan")
+        blob, off = _pack_keys(keys) if keys is not None else (None, None)
+        lblob, loff = _pack_keys(lows) if lows is not None else (None, None)
+        out = np.zeros(max(n * stride, 1), dtype=np.uint8)
+        n_out = np.zeros(max(n, 1), dtype=np.uint32)
+        st = np.zeros(max(n, 1), dtype=np.int32)
+        rc = self.lib.rsp_multi_scan_reverse(self.h, n, _ptr(six), _ptr(blob), _ptr(off), 1 if exclusive else 0,
+                                             _ptr(lblob), _ptr(loff), max_entries, _ptr(out), stride, _ptr(n_out),
+                                             _ptr(st))
+        if rc != OK:
+            raise RuntimeError(f"rsp_multi_scan_reverse -> {rc}")
+        return _scan_records(out, n_out, st, n, stride)
 
     def flush_all(self): return self.lib.rsp_flush_all(self.h)
     def compact_all(self): return self.lib.rsp_compact_all(self.h)
