@@ -265,6 +265,22 @@ int rsp_multi_scan_bounded(rsp_engine* e, size_t n, const uint32_t* shard_ix, co
 int rsp_multi_scan_reverse(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
                            int exclusive, const uint8_t* lows, const uint64_t* loff, uint32_t max_entries,
                            uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st);
+/* Batched scans at snapshots: scan i reads snaps[i] (snapshots of any shards of this engine) and returns what that
+ * snapshot held, whatever writes, flushes, merges or ingestion happened to the shard since.  A NULL or foreign handle
+ * answers InvalidArgument (n_out[i] = 0) for its scan alone.  The scans read the snapshot's pinned runs: they flush no
+ * memtable, create no run, leave rsp_get_stats unchanged and do not answer RSP_BUSY for ticks in flight; they run on
+ * the engine stream under the engine lock.  Records, n_out, st and the host-folded-operator rule are those of
+ * rsp_multi_scan.
+ * rsp_multi_scan_at: forward from the first key >= key i (> key i when exclusive != 0, which continues a page after its
+ * last key; keys == NULL: from the snapshot's first key, and koff is not read), stopping before the exclusive end key
+ * ends[eoff[i] .. eoff[i+1]) as rsp_multi_scan_bounded does (ends == NULL: no end).
+ * rsp_multi_scan_reverse_at: the contract of rsp_multi_scan_reverse (keys == NULL: from the snapshot's last key). */
+int rsp_multi_scan_at(rsp_engine* e, size_t n, rsp_snapshot* const* snaps, const uint8_t* keys, const uint64_t* koff,
+                      int exclusive, const uint8_t* ends, const uint64_t* eoff, uint32_t max_entries,
+                      uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st);
+int rsp_multi_scan_reverse_at(rsp_engine* e, size_t n, rsp_snapshot* const* snaps, const uint8_t* keys,
+                              const uint64_t* koff, int exclusive, const uint8_t* lows, const uint64_t* loff,
+                              uint32_t max_entries, uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st);
 
 /* ---- maintenance: DB::Flush / ApplicationDB::CompactRange(nullptr, nullptr)
  * (application_db.cpp:138-144; triggers admin_handler.cpp:1846,2174) -------------------------------- */
@@ -309,6 +325,19 @@ int rsp_multi_scan_reverse_device(rsp_engine* e, size_t n, const uint32_t* d_sha
                                   uint32_t klen, int exclusive, const uint8_t* d_lows, uint32_t low_klen,
                                   uint32_t max_entries, uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out,
                                   int32_t* d_st, void* stream);
+/* rsp_multi_scan_at / rsp_multi_scan_reverse_at on device pointers: scan i reads the snapshot whose slot
+ * (rsp_snapshot_slot) is d_slot[i]; a slot that holds no snapshot answers InvalidArgument with d_n_out[i] = 0.  Start
+ * key i is d_keys[i*klen .. +klen) (d_keys == NULL: from the snapshot's first / last key), end or low key i
+ * d_ends[i*end_klen .. +end_klen) (NULL: none).  Records and statuses are those of the device form above.  A snapshot's
+ * view is complete (its memtable was sorted into a run when it was taken), so nothing needs flushing first.  The caller
+ * must not release a snapshot while its launches are in flight. */
+int rsp_multi_scan_at_device(rsp_engine* e, size_t n, const uint32_t* d_slot, const uint8_t* d_keys, uint32_t klen,
+                             int exclusive, const uint8_t* d_ends, uint32_t end_klen, uint32_t max_entries,
+                             uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st, void* stream);
+int rsp_multi_scan_reverse_at_device(rsp_engine* e, size_t n, const uint32_t* d_slot, const uint8_t* d_keys,
+                                     uint32_t klen, int exclusive, const uint8_t* d_lows, uint32_t low_klen,
+                                     uint32_t max_entries, uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out,
+                                     int32_t* d_st, void* stream);
 /* One apply tick from a pre-staged device image (see rsp_stage_*): decode + sequence + insert.
  * Memtable capacity must have been reserved with rsp_reserve. */
 typedef struct rsp_staged rsp_staged;

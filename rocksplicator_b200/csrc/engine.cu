@@ -3004,26 +3004,38 @@ int rsp_multi_get_at_device(rsp_engine* e, size_t n, const uint32_t* d_slot, con
 
 // ---- batched scans (host buffers) ----
 // rsp_multi_scan / rsp_multi_scan_bounded / rsp_multi_scan_reverse (ends == nullptr: no end keys; for reverse scans
-// the ends are the lows, and keys == nullptr starts every scan at the shard's last key)
-static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
-                           const uint8_t* ends, const uint64_t* eoff, bool reverse, bool exclusive,
-                           uint32_t max_entries, uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st) {
-  const bool from_last = reverse && !keys;
-  if (!e || (n && (!shard_ix || (!koff && !from_last) || !out || !n_out || !st || (ends && !eoff))))
+// the ends are the lows, and keys == nullptr starts every scan at the shard's last key).  snaps != nullptr:
+// rsp_multi_scan_at / rsp_multi_scan_reverse_at -- scan i reads the pinned view of snaps[i] (shard_ix is not read),
+// keys == nullptr starts every scan at the snapshot's first (forward) or last (reverse) key, and no shard is touched:
+// no flush, no Busy for ticks in flight.
+static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, rsp_snapshot* const* snaps,
+                           const uint8_t* keys, const uint64_t* koff, const uint8_t* ends, const uint64_t* eoff,
+                           bool reverse, bool exclusive, uint32_t max_entries, uint8_t* out, size_t out_stride,
+                           uint32_t* n_out, int32_t* st) {
+  const bool at = snaps != nullptr, from_extreme = !keys && (reverse || at);
+  if (!e || (n && ((!shard_ix && !at) || (!koff && !from_extreme) || !out || !n_out || !st || (ends && !eoff))))
     return RSP_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(e->mu);
   CUDA_OK(cudaSetDevice(e->device));
   if (n == 0) return RSP_OK;
-  std::vector<rsp_shard*> fl;
-  for (size_t i = 0; i < n; i++) {
-    if (shard_ix[i] >= e->slots.size() || !e->slots[shard_ix[i]]) return RSP_INVALID_ARGUMENT;
-    rsp_shard* s = e->slots[shard_ix[i]];
-    if (ticks_in_flight(s)) return RSP_BUSY;
-    if (s->h.mt_count && std::find(fl.begin(), fl.end(), s) == fl.end()) fl.push_back(s);
+  std::vector<u32> slot;
+  if (at) {
+    // a NULL or foreign handle gets a slot the kernel refuses: InvalidArgument for that scan alone
+    slot.resize(n);
+    for (size_t i = 0; i < n; i++) slot[i] = snaps[i] && snaps[i]->s->eng == e ? snaps[i]->slot : 0xffffffffu;
+    shard_ix = slot.data();
+  } else {
+    std::vector<rsp_shard*> fl;
+    for (size_t i = 0; i < n; i++) {
+      if (shard_ix[i] >= e->slots.size() || !e->slots[shard_ix[i]]) return RSP_INVALID_ARGUMENT;
+      rsp_shard* s = e->slots[shard_ix[i]];
+      if (ticks_in_flight(s)) return RSP_BUSY;
+      if (s->h.mt_count && std::find(fl.begin(), fl.end(), s) == fl.end()) fl.push_back(s);
+    }
+    if (!fl.empty()) compact_shards(e, fl, false);
   }
-  if (!fl.empty()) compact_shards(e, fl, false);
   std::vector<uint64_t> no_keys;
-  if (from_last) { no_keys.assign(n + 1, 0); koff = no_keys.data(); }
+  if (from_extreme) { no_keys.assign(n + 1, 0); koff = no_keys.data(); }
   const size_t key_bytes = (size_t)koff[n], end_bytes = ends ? (size_t)eoff[n] : 0;
   const size_t o_koff = align_up(n * 4, 256), o_keys = o_koff + align_up((n + 1) * 8, 256);
   const size_t o_eoff = o_keys + align_up(key_bytes + 16, 256), o_ends = o_eoff + (ends ? align_up((n + 1) * 8, 256) : 0);
@@ -3036,7 +3048,10 @@ static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, co
   ScanArgs a;
   a.shards = e->d_shards; a.views = nullptr; a.shard_ix = (const u32*)d; a.keys = d + o_keys;
   a.koff = (const u64*)(d + o_koff); a.klen_fixed = 0; a.max_entries = max_entries;
-  a.flags = (exclusive ? SCAN_EXCLUSIVE : 0u) | (from_last ? SCAN_FROM_EXTREME : 0u);
+  a.flags = (exclusive ? SCAN_EXCLUSIVE : 0u) | (from_extreme ? SCAN_FROM_EXTREME : 0u);
+  if (at) {
+    a.views = e->d_snap_views; a.n_views = e->d_snap_views ? RSP_MAX_SNAPSHOTS : 0; a.flags |= SCAN_AT_SLOT;
+  }
   a.out = d + o_out; a.out_stride = out_stride; a.n_out = (u32*)(d + o_nout); a.st = (i32*)(d + o_st); a.n = (u32)n;
   if (ends) {
     CUDA_OK(cudaMemcpyAsync(d + o_eoff, eoff, (n + 1) * 8, cudaMemcpyHostToDevice, e->st));
@@ -3075,24 +3090,42 @@ static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, co
 int rsp_multi_scan(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
                    uint32_t max_entries, uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st) {
   try {
-    return multi_scan_host(e, n, shard_ix, keys, koff, nullptr, nullptr, false, false, max_entries, out, out_stride,
-                           n_out, st);
+    return multi_scan_host(e, n, shard_ix, nullptr, keys, koff, nullptr, nullptr, false, false, max_entries, out,
+                           out_stride, n_out, st);
   } catch (...) { return abi_caught(); }
 }
 int rsp_multi_scan_bounded(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
                            const uint8_t* ends, const uint64_t* eoff, uint32_t max_entries, uint8_t* out,
                            size_t out_stride, uint32_t* n_out, int32_t* st) {
   try {
-    return multi_scan_host(e, n, shard_ix, keys, koff, ends, eoff, false, false, max_entries, out, out_stride, n_out,
-                           st);
+    return multi_scan_host(e, n, shard_ix, nullptr, keys, koff, ends, eoff, false, false, max_entries, out, out_stride,
+                           n_out, st);
   } catch (...) { return abi_caught(); }
 }
 int rsp_multi_scan_reverse(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uint8_t* keys, const uint64_t* koff,
                            int exclusive, const uint8_t* lows, const uint64_t* loff, uint32_t max_entries,
                            uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st) {
   try {
-    return multi_scan_host(e, n, shard_ix, keys, koff, lows, loff, true, exclusive != 0, max_entries, out, out_stride,
-                           n_out, st);
+    return multi_scan_host(e, n, shard_ix, nullptr, keys, koff, lows, loff, true, exclusive != 0, max_entries, out,
+                           out_stride, n_out, st);
+  } catch (...) { return abi_caught(); }
+}
+int rsp_multi_scan_at(rsp_engine* e, size_t n, rsp_snapshot* const* snaps, const uint8_t* keys, const uint64_t* koff,
+                      int exclusive, const uint8_t* ends, const uint64_t* eoff, uint32_t max_entries, uint8_t* out,
+                      size_t out_stride, uint32_t* n_out, int32_t* st) {
+  try {
+    if (n && !snaps) return RSP_INVALID_ARGUMENT;
+    return multi_scan_host(e, n, nullptr, snaps, keys, koff, ends, eoff, false, exclusive != 0, max_entries, out,
+                           out_stride, n_out, st);
+  } catch (...) { return abi_caught(); }
+}
+int rsp_multi_scan_reverse_at(rsp_engine* e, size_t n, rsp_snapshot* const* snaps, const uint8_t* keys,
+                              const uint64_t* koff, int exclusive, const uint8_t* lows, const uint64_t* loff,
+                              uint32_t max_entries, uint8_t* out, size_t out_stride, uint32_t* n_out, int32_t* st) {
+  try {
+    if (n && !snaps) return RSP_INVALID_ARGUMENT;
+    return multi_scan_host(e, n, nullptr, snaps, keys, koff, lows, loff, true, exclusive != 0, max_entries, out,
+                           out_stride, n_out, st);
   } catch (...) { return abi_caught(); }
 }
 
@@ -3122,21 +3155,25 @@ int rsp_multi_get_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, co
 
 // rsp_multi_scan_device / rsp_multi_scan_bounded_device / rsp_multi_scan_reverse_device (d_ends == nullptr: no end
 // keys; for reverse scans the ends are the lows, and d_keys == nullptr starts every scan at the shard's last key)
-static int multi_scan_dev(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys, uint32_t klen,
-                          const uint8_t* d_ends, uint32_t end_klen, bool reverse, bool exclusive, uint32_t max_entries,
-                          uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st, void* stream) {
-  const bool from_last = reverse && !d_keys;
-  if (!e || (!klen && !from_last)) return RSP_INVALID_ARGUMENT;
+// at: rsp_multi_scan_at_device / rsp_multi_scan_reverse_at_device -- d_shard_ix holds snapshot table slots, and
+// d_keys == nullptr starts every scan at the snapshot's first (forward) or last (reverse) key
+static int multi_scan_dev(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, bool at, const uint8_t* d_keys,
+                          uint32_t klen, const uint8_t* d_ends, uint32_t end_klen, bool reverse, bool exclusive,
+                          uint32_t max_entries, uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st,
+                          void* stream) {
+  const bool from_extreme = !d_keys && (reverse || at);
+  if (!e || (!klen && !from_extreme)) return RSP_INVALID_ARGUMENT;
   ScanArgs a;
   a.shards = e->d_shards; a.views = nullptr; a.shard_ix = d_shard_ix; a.keys = d_keys; a.koff = nullptr;
-  a.klen_fixed = from_last ? 1u : klen;  // (from the last key: the keys are not read)
-  a.flags = (exclusive ? SCAN_EXCLUSIVE : 0u) | (from_last ? SCAN_FROM_EXTREME : 0u);
+  a.klen_fixed = from_extreme ? 1u : klen;  // (from the first / last key: the keys are not read)
+  a.flags = (exclusive ? SCAN_EXCLUSIVE : 0u) | (from_extreme ? SCAN_FROM_EXTREME : 0u) | (at ? SCAN_AT_SLOT : 0u);
   a.max_entries = max_entries; a.out = d_out; a.out_stride = out_stride;
   a.n_out = d_n_out; a.st = d_st; a.n = (u32)n;
   a.ends = d_ends; a.elen = end_klen;
   {
     std::lock_guard<std::mutex> g(e->mu);
     cudaStream_t rs = stream ? (cudaStream_t)stream : e->st;
+    if (at) { a.views = e->d_snap_views; a.n_views = e->d_snap_views ? RSP_MAX_SNAPSHOTS : 0; }
     reader_begin(e, rs);
     launch_multi_scan(a, reverse, rs);
     reader_end(e, rs);
@@ -3148,15 +3185,15 @@ int rsp_multi_scan_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, c
                           uint32_t max_entries, uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st,
                           void* stream) {
   try {
-    return multi_scan_dev(e, n, d_shard_ix, d_keys, klen, nullptr, 0, false, false, max_entries, d_out, out_stride,
-                          d_n_out, d_st, stream);
+    return multi_scan_dev(e, n, d_shard_ix, false, d_keys, klen, nullptr, 0, false, false, max_entries, d_out,
+                          out_stride, d_n_out, d_st, stream);
   } catch (...) { return abi_caught(); }
 }
 int rsp_multi_scan_bounded_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, const uint8_t* d_keys,
                                   uint32_t klen, const uint8_t* d_ends, uint32_t end_klen, uint32_t max_entries,
                                   uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st, void* stream) {
   try {
-    return multi_scan_dev(e, n, d_shard_ix, d_keys, klen, d_ends, end_klen, false, false, max_entries, d_out,
+    return multi_scan_dev(e, n, d_shard_ix, false, d_keys, klen, d_ends, end_klen, false, false, max_entries, d_out,
                           out_stride, d_n_out, d_st, stream);
   } catch (...) { return abi_caught(); }
 }
@@ -3165,7 +3202,24 @@ int rsp_multi_scan_reverse_device(rsp_engine* e, size_t n, const uint32_t* d_sha
                                   uint32_t max_entries, uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out,
                                   int32_t* d_st, void* stream) {
   try {
-    return multi_scan_dev(e, n, d_shard_ix, d_keys, klen, d_lows, low_klen, true, exclusive != 0, max_entries, d_out,
+    return multi_scan_dev(e, n, d_shard_ix, false, d_keys, klen, d_lows, low_klen, true, exclusive != 0, max_entries,
+                          d_out, out_stride, d_n_out, d_st, stream);
+  } catch (...) { return abi_caught(); }
+}
+int rsp_multi_scan_at_device(rsp_engine* e, size_t n, const uint32_t* d_slot, const uint8_t* d_keys, uint32_t klen,
+                             int exclusive, const uint8_t* d_ends, uint32_t end_klen, uint32_t max_entries,
+                             uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out, int32_t* d_st, void* stream) {
+  try {
+    return multi_scan_dev(e, n, d_slot, true, d_keys, klen, d_ends, end_klen, false, exclusive != 0, max_entries, d_out,
+                          out_stride, d_n_out, d_st, stream);
+  } catch (...) { return abi_caught(); }
+}
+int rsp_multi_scan_reverse_at_device(rsp_engine* e, size_t n, const uint32_t* d_slot, const uint8_t* d_keys,
+                                     uint32_t klen, int exclusive, const uint8_t* d_lows, uint32_t low_klen,
+                                     uint32_t max_entries, uint8_t* d_out, uint64_t out_stride, uint32_t* d_n_out,
+                                     int32_t* d_st, void* stream) {
+  try {
+    return multi_scan_dev(e, n, d_slot, true, d_keys, klen, d_lows, low_klen, true, exclusive != 0, max_entries, d_out,
                           out_stride, d_n_out, d_st, stream);
   } catch (...) { return abi_caught(); }
 }

@@ -184,13 +184,14 @@ constexpr u32 SCAN_VLEN_MERGE_FAILED = 0xfffffffeu;  // the merge failed: empty 
 constexpr i32 SCAN_ST_TRUNCATED = 1 << 30;
 struct ScanArgs {
   const ShardDev* shards;   // used when views == nullptr (shard_ix indexes it)
-  const ScanView* views;    // or explicit pinned views (one per request)
-  const u32* shard_ix;
+  const ScanView* views;    // or explicit pinned views: one per request, or the snapshot table (SCAN_AT_SLOT)
+  const u32* shard_ix;      // (SCAN_AT_SLOT: the snapshot table slot of each request)
   const u8* keys;
   const u64* koff;
   u32 klen_fixed;
-  u32 flags;                // every request: SCAN_EXCLUSIVE, SCAN_FROM_EXTREME
+  u32 flags;                // every request: SCAN_EXCLUSIVE, SCAN_FROM_EXTREME, SCAN_AT_SLOT
   u32 max_entries;
+  u32 n_views = 0;          // SCAN_AT_SLOT: table capacity (0 = no table yet); other slots answer InvalidArgument
   u8* out;
   u64 out_stride;
   u32* n_out;
@@ -205,6 +206,9 @@ struct ScanArgs {
 };
 constexpr u32 SCAN_EXCLUSIVE = 1;      // start after the key (forward: > key; reverse: < key)
 constexpr u32 SCAN_FROM_EXTREME = 2;   // ignore the keys: start at the first (forward) or last (reverse) key
+// request q reads the snapshot table entry views[shard_ix[q]]; a slot >= n_views or not live answers InvalidArgument
+// with n_out = 0
+constexpr u32 SCAN_AT_SLOT = 4;
 // reverse: Iterator::SeekForPrev + Prev (descending keys); otherwise Seek + Next
 void launch_multi_scan(const ScanArgs& a, bool reverse, cudaStream_t s);
 

@@ -102,6 +102,11 @@ EXPORTS = {
     "rsp_multi_scan_reverse": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                          C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p,
                                          C.c_void_p]),
+    "rsp_multi_scan_at": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p,
+                                    C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
+    "rsp_multi_scan_reverse_at": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                            C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_size_t, C.c_void_p,
+                                            C.c_void_p]),
     "rsp_flush": (C.c_int, [C.c_void_p]),
     "rsp_compact": (C.c_int, [C.c_void_p]),
     "rsp_flush_all": (C.c_int, [C.c_void_p]),
@@ -119,6 +124,12 @@ EXPORTS = {
     "rsp_multi_scan_reverse_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int,
                                                 C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p,
                                                 C.c_void_p, C.c_void_p]),
+    "rsp_multi_scan_at_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_int,
+                                           C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p,
+                                           C.c_void_p, C.c_void_p]),
+    "rsp_multi_scan_reverse_at_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32,
+                                                   C.c_int, C.c_void_p, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p]),
     "rsp_stage_build": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                   C.POINTER(C.c_void_p)]),
     "rsp_stage_free": (None, [C.c_void_p]),
@@ -522,6 +533,35 @@ class Engine:
         if rc != OK:
             raise RuntimeError(f"rsp_multi_scan_reverse -> {rc}")
         return _scan_records(out, n_out, st, n, stride)
+
+    def _scan_at(self, fn, snapshots, keys, max_entries, stride, ends, exclusive):
+        n = len(snapshots)
+        if keys is not None and len(keys) != n:
+            raise ValueError("one start key per scan")
+        if ends is not None and len(ends) != n:
+            raise ValueError("one end key per scan")
+        handles = (C.c_void_p * max(n, 1))(*[s.h if s is not None else None for s in snapshots])
+        blob, off = _pack_keys(keys) if keys is not None else (None, None)
+        eblob, eoff = _pack_keys(ends) if ends is not None else (None, None)
+        out = np.zeros(max(n * stride, 1), dtype=np.uint8)
+        n_out = np.zeros(max(n, 1), dtype=np.uint32)
+        st = np.zeros(max(n, 1), dtype=np.int32)
+        rc = getattr(self.lib, fn)(self.h, n, handles, _ptr(blob), _ptr(off), 1 if exclusive else 0, _ptr(eblob),
+                                   _ptr(eoff), max_entries, _ptr(out), stride, _ptr(n_out), _ptr(st))
+        if rc != OK:
+            raise RuntimeError(f"{fn} -> {rc}")
+        return _scan_records(out, n_out, st, n, stride)
+
+    def multi_scan_at(self, snapshots, keys, max_entries, stride, ends=None, exclusive=False):
+        """scan i at snapshots[i] (a Snapshot, or None: InvalidArgument): up to max_entries live entries from keys[i]
+        (after it when exclusive; keys=None: from the snapshot's first key), before ends[i] (exclusive) when ends is
+        given -> [(status, [(key, value)])].  Flushes nothing."""
+        return self._scan_at("rsp_multi_scan_at", snapshots, keys, max_entries, stride, ends, exclusive)
+
+    def multi_scan_reverse_at(self, snapshots, keys, max_entries, stride, lows=None, exclusive=False):
+        """multi_scan_reverse at snapshots[i] (keys=None: from the snapshot's last key) -> [(status, [(key, value)])].
+        Flushes nothing."""
+        return self._scan_at("rsp_multi_scan_reverse_at", snapshots, keys, max_entries, stride, lows, exclusive)
 
     def flush_all(self): return self.lib.rsp_flush_all(self.h)
     def compact_all(self): return self.lib.rsp_compact_all(self.h)
