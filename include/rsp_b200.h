@@ -43,13 +43,18 @@ enum rsp_status {
   RSP_BUSY = 11
 };
 
-/* merge operators that run on the device; anything else is folded on the host through a callback */
+/* merge operators.  The counter, uint64add and string append run on the device (reads, flushes and merges fold them
+ * there); RSP_MERGE_APPEND and RSP_MERGE_CALLBACK are folded on the host. */
 enum rsp_merge_op {
   RSP_MERGE_NONE = 0,      /* Merge records are stored; reads answer InvalidArgument as RocksDB does */
   RSP_MERGE_COUNTER = 1,   /* examples/counter_service/merge_operator.cpp:23-45 (int64 LE add) */
   RSP_MERGE_UINT64ADD = 2, /* RocksDB built-in "uint64add" (malformed operand == 0) */
   RSP_MERGE_APPEND = 3,    /* rocksdb_replicator/tests/rocksdb_assumption_test.cpp:58-77 (host fold) */
-  RSP_MERGE_CALLBACK = 4   /* rsp_shard_opts.merge_fn (host fold) */
+  RSP_MERGE_CALLBACK = 4,  /* rsp_shard_opts.merge_fn (host fold) */
+  RSP_MERGE_STRING_APPEND = 5 /* RocksDB's StringAppendOperator: existing + delimiter + operand, operands oldest first;
+                               * no existing value (nothing, Delete, SingleDelete): the operand.  A Put of "" is an
+                               * existing value.  Never fails.  The delimiter is rsp_shard_opts.merge_delim.  No read,
+                               * scan or device form answers 100 or the host-fold record marker for it. */
 };
 
 typedef struct rsp_engine rsp_engine; /* one per GPU */
@@ -74,7 +79,8 @@ typedef struct rsp_engine_cfg {
 
 typedef struct rsp_shard_opts {
   uint32_t merge_op;          /* enum rsp_merge_op */
-  uint32_t reserved;
+  uint32_t merge_delim;       /* RSP_MERGE_STRING_APPEND: 0 = no delimiter, 0x100 | c = the byte c (c may be 0); any
+                               * other bit answers InvalidArgument.  Other operators ignore it. */
   uint64_t write_buffer_bytes; /* memtable entry-heap capacity (options.write_buffer_size); 0 = 1 MiB */
   rsp_merge_fn merge_fn;       /* RSP_MERGE_CALLBACK */
   void* merge_state;
@@ -301,7 +307,8 @@ int rsp_ingest_sorted(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_
 /* ---- device-pointer forms (kernel-level measurement; inputs/outputs already in HBM) -------------
  * `stream` is a cudaStream_t passed as void* (0 = the engine's own read stream).  No host
  * synchronisation is performed; the caller owns ordering and timing.  A lookup that needs a host-side merge operator
- * (RSP_MERGE_CALLBACK shards with merge operands on the key) cannot be finished on the device: its d_st is 100 and the
+ * (RSP_MERGE_APPEND / RSP_MERGE_CALLBACK shards with merge operands on the key) cannot be finished on the device: its
+ * d_st is 100 and the
  * caller resolves it with rsp_get / rsp_multi_get.  rsp_multi_scan_device scans the sorted runs only: on a shard whose
  * memtable holds writes it returns the runs' contents with d_st = 0, without those writes.  Flush such shards first, or
  * use rsp_multi_scan, which does.

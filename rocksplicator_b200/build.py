@@ -69,11 +69,13 @@ HOST_SO = os.path.join(HERE, "librsp_host.so")
 HOST_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "host_tests")
 SNAPSHOT_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "snapshot_tests")
 BOUNDED_ITER_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "bounded_iter_tests")
+STRING_APPEND_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "string_append_tests")
 
 
 def build_host(force=False, verbose=False):
-    """The C++ mirror of the reference interfaces (host/) -> librsp_host.so, and its test binaries (snapshot_tests and
-    bounded_iter_tests are returned by build_snapshot_tests and build_bounded_iter_tests)."""
+    """The C++ mirror of the reference interfaces (host/) -> librsp_host.so, and its test binaries (snapshot_tests,
+    bounded_iter_tests and string_append_tests are returned by build_snapshot_tests, build_bounded_iter_tests and
+    build_string_append_tests)."""
     build(force=False, verbose=verbose)
     srcs = [os.path.join(HOST, s) for s in HOST_SRCS]
     deps = list(srcs)
@@ -93,7 +95,7 @@ def build_host(force=False, verbose=False):
     if force or _stale(HOST_TESTS, [tsrc, HOST_SO] + deps):
         run([cxx] + flags + ["-o", HOST_TESTS, tsrc, "-L", HERE, "-lrsp_host", "-lrsp_b200",
                              "-Wl,-rpath," + HERE])
-    for exe in (SNAPSHOT_TESTS, BOUNDED_ITER_TESTS):
+    for exe in (SNAPSHOT_TESTS, BOUNDED_ITER_TESTS, STRING_APPEND_TESTS):
         src = exe + ".cpp"
         if force or _stale(exe, [src, HOST_SO] + deps):
             run([cxx] + flags + ["-o", exe, src, "-L", HERE, "-lrsp_host", "-lrsp_b200", "-Wl,-rpath," + HERE])
@@ -111,3 +113,10 @@ def build_bounded_iter_tests(force=False, verbose=False):
     SeekForPrev"""
     build_host(force=force, verbose=verbose)
     return BOUNDED_ITER_TESTS
+
+
+def build_string_append_tests(force=False, verbose=False):
+    """tests/cpp/string_append_tests: rocksdb::StringAppendOperator through GpuDB / ApplicationDB (the device operator,
+    reads at snapshots, Backup / Restore)"""
+    build_host(force=force, verbose=verbose)
+    return STRING_APPEND_TESTS

@@ -264,6 +264,8 @@ struct rsp_engine {
   ShardFast* d_fast_runs = nullptr;
   u32* d_mt_filter = nullptr;  // behind d_fast_runs in the same allocation (format.cuh: memtable filter)
   std::atomic<u32> n_multirun{0};
+  // open RSP_MERGE_STRING_APPEND shards: while there is one, reads launch the kernel instances with that fold
+  std::atomic<u32> n_string_append{0};
   struct Compactor* compactor = nullptr;
   u32 mg_parity = 0;
   size_t pending_cap = 0;
@@ -504,6 +506,7 @@ static void plan_jobs(rsp_engine* e, const std::vector<rsp_shard*>& shards, Comp
     j.n_tiles = ns > 1 ? (u32)((n + MERGE_TILE - 1) / MERGE_TILE) : 0;
     j.bottom = (full && mode != COMPACT_SNAPSHOT) ? 1 : 0;
     j.merge_op = s->opts.merge_op;
+    j.merge_delim = s->h.merge_delim;
     h.items_b = (size_t)std::max<u32>(1, j.items_len) * sizeof(SortItem);
     h.items2_b = ns > 1 ? (size_t)std::max<u32>(1, j.n_items) * sizeof(SortItem) : 0;
     h.coranks_b = ns > 1 ? (size_t)(j.n_tiles + 1) * ns * 4 : 0;
@@ -696,6 +699,7 @@ static void view_of(const rsp_shard* s, const std::vector<std::shared_ptr<Run>>&
   memset(v, 0, sizeof(*v));
   v->n_runs = (u32)pinned.size();
   v->merge_op = s->opts.merge_op;
+  v->merge_delim = s->h.merge_delim;
   for (u32 i = 0; i < v->n_runs; i++) v->runs[i] = pinned[i]->dev();
 }
 
@@ -1409,6 +1413,9 @@ static void set_pending(rsp_engine* e, GetArgs& a, size_t n, cudaStream_t stream
   e->mg_parity ^= 1u;
 }
 
+// the read kernels' instances with the string-append fold are launched while a shard of the engine needs it
+static bool cat_reads(const rsp_engine* e) { return e->n_string_append.load() != 0; }
+
 // the fields of a MultiGet launch the engine owns: the shard descriptors, and whether some shard has several runs
 static void set_engine_args(rsp_engine* e, GetArgs& a) {
   a.shards = e->d_shards; a.fast = e->d_fast; a.max_shards = e->cfg.max_shards;
@@ -1498,7 +1505,7 @@ static int multi_get_locked(rsp_engine* e, size_t n, const uint32_t* shard_ix, c
     a.vals = d + o_vals + c0 * val_stride; a.val_stride = val_stride;
     a.vlen = (u32*)(d + o_vlen) + c0; a.st = (i32*)(d + o_st) + c0; a.n = (u32)cn;
     a.n_special = scratch; a.n_pending = scratch + 4 + 2 * c; a.pending = scratch + 4 + 2 * n_chunks + c0; a.parity = 0;
-    if (launch_multi_get(a, cs)) e->last_mg.fast = true;
+    if (launch_multi_get(a, cat_reads(e), cs)) e->last_mg.fast = true;
     e->launches += 2;
     CUDA_OK(cudaMemcpyAsync(vlen + c0, d + o_vlen + c0 * 4, cn * 4, cudaMemcpyDeviceToHost, cs));
     CUDA_OK(cudaMemcpyAsync(st + c0, d + o_st + c0 * 4, cn * 4, cudaMemcpyDeviceToHost, cs));
@@ -1583,7 +1590,7 @@ static void iter_fetch(rsp_iter* it, const std::string* key, bool exclusive, boo
       if (elen) CUDA_OK(cudaMemcpyAsync(d + o_ekey, it->upper.data(), elen, cudaMemcpyHostToDevice, e->st));
       a.ends = d + o_ekey; a.eoff = (const u64*)(d + 40);
     }
-    launch_multi_scan(a, reverse, e->st);
+    launch_multi_scan(a, reverse, it->s->opts.merge_op == RSP_MERGE_STRING_APPEND, e->st);
     e->launches++;
     u32 res[2];
     CUDA_OK(cudaMemcpyAsync(res, d + 32, 8, cudaMemcpyDeviceToHost, e->st));
@@ -1766,7 +1773,7 @@ struct ReadCombiner {
       // ordering against flushes / memtable re-allocations on the engine stream (reader_begin / reader_end)
       std::lock_guard<std::mutex> g(e->mu);
       reader_begin(e, stream);
-      launch_multi_get(a, stream);
+      launch_multi_get(a, cat_reads(e), stream);
       CUDA_OK(cudaGetLastError());
       reader_end(e, stream);
     }
@@ -2130,6 +2137,7 @@ void* rsp_engine_stream(const rsp_engine* e) { return (void*)e->st; }
 
 static int shard_open_locked(rsp_engine* e, const char* name, const rsp_shard_opts* opts, rsp_shard** out) {
   if (e->by_name.count(name)) return RSP_INVALID_ARGUMENT;
+  if (opts && opts->merge_op == RSP_MERGE_STRING_APPEND && (opts->merge_delim & ~0x1ffu)) return RSP_INVALID_ARGUMENT;
   u32 ix = 0;
   while (ix < e->slots.size() && e->slots[ix]) ix++;
   if (ix >= e->cfg.max_shards) return RSP_BUSY;
@@ -2142,12 +2150,14 @@ static int shard_open_locked(rsp_engine* e, const char* name, const rsp_shard_op
   if (opts) s->opts = *opts;
   memset(&s->h, 0, sizeof(s->h));
   s->h.merge_op = s->opts.merge_op;
+  s->h.merge_delim = s->opts.merge_op == RSP_MERGE_STRING_APPEND ? s->opts.merge_delim : 0u;
   s->h.live = 1;
   alloc_memtable(e, s, 0, 0);
   UploadBatch up;
   stage_upload(e, s, false, true, &up);
   commit_uploads(e, &up);
   CUDA_OK(cudaStreamSynchronize(e->st));
+  if (s->opts.merge_op == RSP_MERGE_STRING_APPEND) e->n_string_append++;
   e->slots[ix] = s;
   e->by_name[name] = s;
   *out = s;
@@ -2161,6 +2171,7 @@ static void shard_close_locked(rsp_shard* s) {
   e->slots[s->index] = nullptr;
   e->by_name.erase(s->name);
   if (s->counted_multirun) { e->n_multirun--; s->counted_multirun = false; }
+  if (s->opts.merge_op == RSP_MERGE_STRING_APPEND) e->n_string_append--;
   ShardDev z;
   memset(&z, 0, sizeof(z));
   CUDA_OK(cudaMemcpy(e->d_shards + s->index, &z, sizeof(z), cudaMemcpyHostToDevice));
@@ -2932,7 +2943,7 @@ static int multi_get_at_locked(rsp_engine* e, size_t n, rsp_snapshot* const* sna
   a.vals = d + o_vals; a.val_stride = val_stride; a.vlen = (u32*)(d + o_vlen); a.st = (i32*)(d + o_st);
   a.n_special = (u32*)(d + o_spec); a.n_views = e->d_snap_views ? RSP_MAX_SNAPSHOTS : 0; a.klen_fixed = 0; a.n = (u32)n;
   CUDA_OK(cudaEventRecord(e->ev0, e->st));
-  launch_multi_get_at(a, e->st);
+  launch_multi_get_at(a, cat_reads(e), e->st);
   CUDA_OK(cudaGetLastError());
   e->launches++;
   CUDA_OK(cudaEventRecord(e->ev1, e->st));
@@ -2994,7 +3005,7 @@ int rsp_multi_get_at_device(rsp_engine* e, size_t n, const uint32_t* d_slot, con
     a.views = e->d_snap_views;
     a.n_views = e->d_snap_views ? RSP_MAX_SNAPSHOTS : 0;
     reader_begin(e, rs);
-    launch_multi_get_at(a, rs);
+    launch_multi_get_at(a, cat_reads(e), rs);
     reader_end(e, rs);
   }
   e->launches++;
@@ -3059,7 +3070,7 @@ static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, rs
     a.ends = d + o_ends; a.eoff = (const u64*)(d + o_eoff);
   }
   CUDA_OK(cudaEventRecord(e->ev0, e->st));
-  launch_multi_scan(a, reverse, e->st);
+  launch_multi_scan(a, reverse, cat_reads(e), e->st);
   e->launches++;
   CUDA_OK(cudaEventRecord(e->ev1, e->st));
   CUDA_OK(cudaMemcpyAsync(n_out, d + o_nout, n * 4, cudaMemcpyDeviceToHost, e->st));
@@ -3143,7 +3154,7 @@ int rsp_multi_get_device(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, co
     set_pending(e, a, n, rs);
     reader_begin(e, rs);
     set_engine_args(e, a);
-    e->last_mg.fast = launch_multi_get(a, rs);
+    e->last_mg.fast = launch_multi_get(a, cat_reads(e), rs);
     e->last_mg.host = false; e->last_mg.parity = a.parity; e->last_mg.n_chunks = 1; e->last_mg.chunk = n;
     reader_end(e, rs);
     pending_mark(e, rs);
@@ -3175,7 +3186,7 @@ static int multi_scan_dev(rsp_engine* e, size_t n, const uint32_t* d_shard_ix, b
     cudaStream_t rs = stream ? (cudaStream_t)stream : e->st;
     if (at) { a.views = e->d_snap_views; a.n_views = e->d_snap_views ? RSP_MAX_SNAPSHOTS : 0; }
     reader_begin(e, rs);
-    launch_multi_scan(a, reverse, rs);
+    launch_multi_scan(a, reverse, cat_reads(e), rs);
     reader_end(e, rs);
   }
   e->launches++;

@@ -92,6 +92,10 @@ constexpr u32 RUN_BUCKET_SLOTS = 8;    // u32 slots per hash bucket = one 32 B s
 // internal lookup results beyond rocksdb codes
 constexpr i32 ST_NEED_HOST_MERGE = 100;
 
+// RSP_MERGE_STRING_APPEND: existing + delimiter + operand, folded on the device.  The device also folds the counter (1)
+// and uint64add (2); RSP_MERGE_APPEND (3), RSP_MERGE_CALLBACK (4) and unknown operators are folded on the host.
+constexpr u32 MERGE_OP_STRING_APPEND = 5;
+
 struct __align__(16) RunDev {
   const u8* heap;
   const u32* ent_off;
@@ -124,7 +128,7 @@ struct __align__(16) ShardDev {
   u32 latch;         // mk_status(code,msg) of the latched write error, 0 = healthy
   u32 n_runs;
   u32 live;
-  u32 pad;
+  u32 merge_delim;   // RSP_MERGE_STRING_APPEND: 0 = no delimiter, 0x100 | c = the byte c
   RunDev runs[RSP_MAX_RUNS];  // [0] = newest
 };
 

@@ -13,8 +13,9 @@
 //                     under the strict order key / source / rank), then one CTA per 2048-item tile gathers its
 //                     sub-ranges into shared memory, orders them there and writes the tile — many CTAs per shard
 //   k_compact_size  : per user key: keep what a read can still observe (newest Put; tombstone unless
-//                     bottom-most; Merge operands folded with the device operators, otherwise the
-//                     operand stack down to its base), then an exclusive scan -> output offsets
+//                     bottom-most; Merge operands folded with the device operators — the counter, uint64add and
+//                     string append — otherwise the operand stack down to its base), then an exclusive scan ->
+//                     output offsets
 //   k_compact_write : copy / synthesise the kept entries into the new heap, write the restart array
 //                     (ent_off), the block index (first-key prefix per 32 entries) and the bucketised
 //                     hash index
@@ -28,7 +29,12 @@ namespace rsp {
 constexpr u32 KEEP_UNITS_MASK = 0x00ffffffu;
 constexpr u32 KEEP_HEAD = 1u << 24;
 constexpr u32 KEEP_MODE_SHIFT = 28;
-enum : u32 { MODE_COPY = 0, MODE_PUT_IMM = 1, MODE_PUT_BYTES = 2, MODE_MERGE_IMM = 3 };
+// MODE_PUT_CAT / MODE_MERGE_CAT: a string-append fold, written as one Put / one Merge operand (fold_val: its length << 32
+// | a Put base under the operands << 31 | the operand count)
+enum : u32 { MODE_COPY = 0, MODE_PUT_IMM = 1, MODE_PUT_BYTES = 2, MODE_MERGE_IMM = 3, MODE_PUT_CAT = 4, MODE_MERGE_CAT = 5 };
+constexpr u32 CAT_BASE = 1u << 31;
+// a fold longer than this keeps its operands (reads fold them): its entry would not fit the 24-bit unit count
+constexpr u64 CAT_MAX_LEN = 1ull << 27;
 constexpr u32 PAD_REF = 0xffffffffu;
 
 struct EntView {
@@ -393,6 +399,8 @@ __global__ void __launch_bounds__(1024) k_compact_size(const CompactJob* jobs) {
   const u32 n = j.n_items;
   const SortItem* it = j.sorted;
   const bool foldable = j.merge_op == 1 || j.merge_op == 2;
+  const bool cat = j.merge_op == MERGE_OP_STRING_APPEND;
+  const u32 dl = j.merge_delim ? 1u : 0u;
   for (u32 i = threadIdx.x; i < n; i += blockDim.x) {
     if (i > 0 && same_key(j, it[i - 1], it[i])) continue;  // not the newest version of its key
     // i heads a group of versions of one user key, newest first
@@ -410,11 +418,12 @@ __global__ void __launch_bounds__(1024) k_compact_size(const CompactJob* jobs) {
     } else {
       // operands i .. m-1, optional base at m
       u32 m = i, n_bad = 0;
-      u64 sum = 0;
+      u64 sum = 0, cat_len = 0;
       while (m < g_end) {
         const EntView x = view_item(j, it[m]);
         if (x.type != kTypeMerge) break;
         if (x.vlen == 8) sum += *reinterpret_cast<const u64*>(x.val); else n_bad++;
+        cat_len += x.vlen + dl;
         m++;
       }
       const u32 n_ops = m - i;
@@ -438,9 +447,22 @@ __global__ void __launch_bounds__(1024) k_compact_size(const CompactJob* jobs) {
         } else if (n_ops >= 2 && (j.merge_op == 2 || n_bad == 0)) {  // partial merge of the operands
           folded = true; val = sum; mode = MODE_MERGE_IMM;
         }
+      } else if (cat) {
+        // base d o_1 .. d o_n: a Put on a Put, a Put on a tombstone or at the bottom (no existing value), otherwise
+        // the operands' partial merge o_1 d .. d o_n (associative) as one operand
+        cat_len -= dl;
+        if (base_put) cat_len += base.vlen + dl;
+        if (base_put || has_base_ent || j.bottom) mode = MODE_PUT_CAT;
+        else if (n_ops >= 2) mode = MODE_MERGE_CAT;
+        if (mode != MODE_COPY && cat_len <= CAT_MAX_LEN) {
+          folded = true;
+          val = (cat_len << 32) | (base_put ? CAT_BASE : 0u) | n_ops;
+        }
       }
       if (folded) {
-        const u32 units = mode == MODE_PUT_BYTES ? entry_units(kTypeValue, e0.klen, e0.vlen, false) : imm_units(e0.klen);
+        const u32 units = mode == MODE_PUT_BYTES ? entry_units(kTypeValue, e0.klen, e0.vlen, false)
+                        : mode >= MODE_PUT_CAT ? entry_units(kTypeValue, e0.klen, (u32)(val >> 32), false)
+                                               : imm_units(e0.klen);
         j.keep_units[i] = units | KEEP_HEAD | (mode << KEEP_MODE_SHIFT);
         j.fold_val[i] = val;
       } else {
@@ -477,8 +499,10 @@ __global__ void __launch_bounds__(1024) k_compact_size(const CompactJob* jobs) {
         const EntView x = view_item(j, it[i]);
         x_type = x.type; x_klen = x.klen; x_vlen = x.vlen;
       }
-      const u32 type = (mode == MODE_PUT_IMM || mode == MODE_PUT_BYTES) ? (u32)kTypeValue : (mode == MODE_MERGE_IMM ? (u32)kTypeMerge : x_type);
-      const u32 vlen = (mode == MODE_PUT_IMM || mode == MODE_MERGE_IMM) ? 8u : x_vlen;
+      const u32 type = (mode == MODE_PUT_IMM || mode == MODE_PUT_BYTES || mode == MODE_PUT_CAT) ? (u32)kTypeValue
+                     : (mode == MODE_MERGE_IMM || mode == MODE_MERGE_CAT) ? (u32)kTypeMerge : x_type;
+      const u32 vlen = (mode == MODE_PUT_IMM || mode == MODE_MERGE_IMM) ? 8u
+                     : mode >= MODE_PUT_CAT ? (u32)(j.fold_val[i] >> 32) : x_vlen;
       if (type != kTypeValue || x_klen > 0xffffu || vlen > 0xffffu) np++;
       const u32 kv = (x_klen & 0xffffu) | (vlen << 16);
       kvmin = min(kvmin, kv); kvmax = max(kvmax, kv);
@@ -526,6 +550,21 @@ __device__ __forceinline__ void copy_units(u8* dst, const u8* src, u32 units) {
   if (u < units) d[u] = s[u];
 }
 
+// the value of a string-append fold headed by sorted item i: the Put base under the operands (if any), then the operands
+// oldest first, delimited; the padding of the last unit is zeroed
+__device__ __noinline__ void write_cat(const CompactJob& j, u32 i, u8* out, u32 vlen) {
+  const u64 fv = j.fold_val[i];
+  const u32 n_ops = (u32)fv & ~CAT_BASE;
+  u32 at = 0;
+  for (u32 k = i + n_ops + ((u32)fv & CAT_BASE ? 1u : 0u); k-- > i;) {
+    const EntView x = view_item(j, j.sorted[k]);
+    for (u32 b = 0; b < x.vlen; b++) out[at + b] = x.val[b];
+    at += x.vlen;
+    if (k > i && j.merge_delim) out[at++] = (u8)j.merge_delim;
+  }
+  for (u32 b = vlen; b < units_of(vlen) * 16u; b++) out[b] = 0;
+}
+
 __global__ void __launch_bounds__(256) k_compact_write(const CompactJob* jobs) {
   const CompactJob& j = jobs[blockIdx.y];
   const u32 i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -539,14 +578,18 @@ __global__ void __launch_bounds__(256) k_compact_write(const CompactJob* jobs) {
   u8* d = j.out_heap + (u64)pos * 16u;
   const u32 ku_key = units_of(x.klen);
   u32 type = x.type, vlen = x.vlen;
-  if (mode == MODE_PUT_IMM || mode == MODE_PUT_BYTES) type = kTypeValue;
+  if (mode == MODE_PUT_IMM || mode == MODE_PUT_BYTES || mode == MODE_PUT_CAT) type = kTypeValue;
   if (mode == MODE_PUT_IMM || mode == MODE_MERGE_IMM) vlen = 8;
+  if (mode >= MODE_PUT_CAT) vlen = (u32)(j.fold_val[i] >> 32);
   const u64 st = (x.seqtype & ~0xffull) | type;
   *reinterpret_cast<uint4*>(d) = make_uint4((u32)st, (u32)(st >> 32), x.klen, vlen);
   if (mode == MODE_PUT_IMM || mode == MODE_MERGE_IMM) {
     copy_units(d + 16, reinterpret_cast<const u8*>(x.key), ku_key);
     const u64 v = j.fold_val[i];
     *reinterpret_cast<uint4*>(d + 16u + 16u * ku_key) = make_uint4((u32)v, (u32)(v >> 32), 0u, 0u);
+  } else if (mode >= MODE_PUT_CAT) {
+    copy_units(d + 16, reinterpret_cast<const u8*>(x.key), ku_key);
+    write_cat(j, i, d + 16u + 16u * ku_key, vlen);
   } else {
     // key and value units follow each other in a memtable entry as in a run entry: one copy
     copy_units(d + 16, reinterpret_cast<const u8*>(x.key), ku_key + units_of(x.vlen));

@@ -130,8 +130,10 @@ struct GetArgs {
 };
 static_assert(sizeof(GetArgs) == 128, "GetArgs layout is part of k_multi_get16's measured code generation");
 // true when the 16-byte-key kernel ran (its deferred lookups are in a.pending, counted in a.n_pending[a.parity]);
-// false when the generic kernel served every lookup
-bool launch_multi_get(const GetArgs& a, cudaStream_t s);
+// false when the generic kernel served every lookup.  cat: some shard the launch may read folds with
+// RSP_MERGE_STRING_APPEND (the generic kernels' instances with that fold; the others hand such operands to the host).
+// The same holds for the launches below.
+bool launch_multi_get(const GetArgs& a, bool cat, cudaStream_t s);
 
 // dump the version stack of each key (newest first, up to and including the first Put/Delete) for
 // host-side merge folding: records [u32 type][u32 vlen][value, padded to 4] at out + i*stride
@@ -156,7 +158,7 @@ struct ScanView {
   u32 n_runs;
   u32 merge_op;
   u32 live;  // snapshot table slots: 1 while the snapshot is held (k_multi_get_at answers InvalidArgument otherwise)
-  u32 pad1;
+  u32 merge_delim;  // ShardDev::merge_delim of the shard
 };
 
 // point lookups at snapshots: lookup q walks the pinned view views[slot[q]] (sorted runs only, newest first) with
@@ -175,7 +177,7 @@ struct GetAtArgs {
   u32 klen_fixed;
   u32 n;
 };
-void launch_multi_get_at(const GetAtArgs& a, cudaStream_t s);
+void launch_multi_get_at(const GetAtArgs& a, bool cat, cudaStream_t s);
 // vlen markers in scan records (the value is absent: the record is [u32 klen][u32 marker][key])
 constexpr u32 SCAN_VLEN_HOST_FOLD = 0xffffffffu;     // the merge operator lives on the host: fold this key there
 constexpr u32 SCAN_VLEN_MERGE_FAILED = 0xfffffffeu;  // the merge failed: empty value, the scan's st holds the status
@@ -210,7 +212,7 @@ constexpr u32 SCAN_FROM_EXTREME = 2;   // ignore the keys: start at the first (f
 // with n_out = 0
 constexpr u32 SCAN_AT_SLOT = 4;
 // reverse: Iterator::SeekForPrev + Prev (descending keys); otherwise Seek + Next
-void launch_multi_scan(const ScanArgs& a, bool reverse, cudaStream_t s);
+void launch_multi_scan(const ScanArgs& a, bool reverse, bool cat, cudaStream_t s);
 
 // ---- flush / compaction ---------------------------------------------------------------------------
 struct SortItem {
@@ -232,7 +234,7 @@ struct CompactJob {
   u32 items_len;    // length of items[]: n_pow2 (memtable segment, padded) + the runs' entries
   u32 seg_start[RSP_MAX_RUNS + 1];  // first item of each source's segment in items[]
   u32 n_tiles;      // merge tiles of MERGE_TILE items (n_src > 1)
-  u32 pad;
+  u32 merge_delim;  // ShardDev::merge_delim of the shard
   // work buffers
   SortItem* items;  // [items_len]: one sorted segment per source (the runs are sorted as stored)
   SortItem* items2; // [n_items]: the segments merged (n_src > 1)
@@ -241,7 +243,7 @@ struct CompactJob {
   u32* keep_units;  // [n_items] output size in units of each sorted item (0 = dropped)
   u32* out_pos;     // [n_items] exclusive scan of keep_units
   u32* out_ord;     // [n_items] exclusive scan of (keep_units != 0)
-  u64* fold_val;    // [n_items] folded 8-byte merge results
+  u64* fold_val;    // [n_items] folded 8-byte merge results; string-append folds: length << 32 | base flag << 31 | n_ops
   u32* totals;      // [8]: units, entries, uniform_units (or 0), distinct keys, non-Put entries, min/max klen<<16|vlen..
   // outputs (allocated by the host after the sizing pass)
   u8* out_heap;

@@ -14,7 +14,7 @@ SO_PATH = os.path.join(HERE, "librsp_b200.so")
 
 OK, NOT_FOUND, CORRUPTION, NOT_SUPPORTED, INVALID_ARGUMENT, IO_ERROR = 0, 1, 2, 3, 4, 5
 INCOMPLETE = 7
-MERGE_NONE, MERGE_COUNTER, MERGE_UINT64ADD, MERGE_APPEND, MERGE_CALLBACK = 0, 1, 2, 3, 4
+MERGE_NONE, MERGE_COUNTER, MERGE_UINT64ADD, MERGE_APPEND, MERGE_CALLBACK, MERGE_STRING_APPEND = 0, 1, 2, 3, 4, 5
 
 MERGE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                        C.c_size_t, C.c_void_p, C.c_void_p)
@@ -26,7 +26,7 @@ class EngineCfg(C.Structure):
 
 
 class ShardOpts(C.Structure):
-    _fields_ = [("merge_op", C.c_uint32), ("reserved", C.c_uint32), ("write_buffer_bytes", C.c_uint64),
+    _fields_ = [("merge_op", C.c_uint32), ("merge_delim", C.c_uint32), ("write_buffer_bytes", C.c_uint64),
                 ("merge_fn", C.c_void_p), ("merge_state", C.c_void_p)]
 
 
@@ -177,8 +177,9 @@ def _pack_keys(keys):
 
 def _scan_records(out, n_out, st, n, stride):
     """the [u32 klen][u32 vlen][key][value] records of n scans at out + i * stride -> [(status, [(key, value)])].  A key
-    that needs the host-side merge operator (vlen 0xffffffff, no value bytes; the scan's status is NotSupported) comes
-    back as (key, None)."""
+    that needs a host-side merge operator (RSP_MERGE_APPEND or RSP_MERGE_CALLBACK: vlen 0xffffffff, no value bytes; the
+    scan's status is NotSupported in the host forms, 100 in the device forms) comes back as (key, None).  Device-folded
+    operators (counter, uint64add, string append) always come back with their value."""
     res = []
     for i in range(n):
         recs, at = [], i * stride
@@ -302,11 +303,17 @@ class Shard:
     """One DB ("segment%05d"): apply == DbWrapper::HandleReplicateResponse, write == WriteToLeader,
     latest_seq == LatestSequenceNumber, get/multi_get/iterator == the ApplicationDB read surface."""
 
-    def __init__(self, engine, name, merge_op=MERGE_NONE, write_buffer_bytes=0, merge_fn=None):
+    def __init__(self, engine, name, merge_op=MERGE_NONE, write_buffer_bytes=0, merge_fn=None, merge_delim=None):
+        """merge_delim: MERGE_STRING_APPEND's delimiter, one byte (b"," / b"\\0") or None for plain concatenation"""
         self.engine = engine
         self.lib = engine.lib
         self.kind = "b200"
-        opts = ShardOpts(merge_op=merge_op, write_buffer_bytes=write_buffer_bytes)
+        delim = 0
+        if merge_delim is not None:
+            if len(merge_delim) != 1:
+                raise ValueError("merge_delim is one byte or None")
+            delim = 0x100 | bytes(merge_delim)[0]
+        opts = ShardOpts(merge_op=merge_op, merge_delim=delim, write_buffer_bytes=write_buffer_bytes)
         self._merge_fn = None
         if merge_fn is not None:
             self._merge_fn = MERGE_FN(merge_fn)

@@ -7,6 +7,7 @@
 #include <cstring>
 #include <map>
 
+#include "rocksdb/string_append_operator.h"
 #include "sst/sst_format.h"
 
 namespace b200 {
@@ -52,7 +53,10 @@ Status GpuDB::Open(const rocksdb::Options& options, const std::string& name, roc
   if (options.merge_operator) {
     const std::string n = options.merge_operator->Name();
     // operators whose semantics the device implements exactly; anything else folds on the host through the callback
-    if (n == "CounterMergeOperator") so.merge_op = RSP_MERGE_COUNTER;        // examples/counter_service/merge_operator.cpp
+    // (the string-append operator by its type: its delimiter travels with it)
+    const auto* sa = dynamic_cast<const rocksdb::StringAppendOperator*>(options.merge_operator.get());
+    if (sa) { so.merge_op = RSP_MERGE_STRING_APPEND; so.merge_delim = sa->has_delim() ? 0x100u | (uint8_t)sa->delim() : 0u; }
+    else if (n == "CounterMergeOperator") so.merge_op = RSP_MERGE_COUNTER;   // examples/counter_service/merge_operator.cpp
     else if (n == "UInt64AddOperator") so.merge_op = RSP_MERGE_UINT64ADD;    // RocksDB built-in
     else { so.merge_op = RSP_MERGE_CALLBACK; so.merge_fn = &GpuDB::MergeTrampoline; so.merge_state = options.merge_operator.get(); }
   }
