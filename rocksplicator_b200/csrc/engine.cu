@@ -1320,29 +1320,36 @@ static bool host_merge_one(rsp_shard* s, const std::string& key, bool has, const
   }
 }
 
+// The device scratch of a host-form read (e->dev_q, shared by all of them): add() hands out the offsets of its pieces
+// front to back, each on a 256-byte boundary; dev_q.get(size) is taken once every piece is laid out (it may move).
+struct QLayout {
+  size_t size = 0;
+  size_t add(size_t bytes) { const size_t o = size; size += align_up(bytes, 256); return o; }
+};
+
 // resolve one key through the version-dump kernel and the host operator
 static int host_fold_get(rsp_engine* e, rsp_shard* s, const uint8_t* key, size_t klen, std::string* value,
                          const ScanView* d_view = nullptr) {
   size_t stride = 4096;
   for (;;) {
-    u8* d = (u8*)e->dev_q.get(klen + 64 + stride + 64);
-    u64 koff[2] = {0, klen};
-    u32 six = s->index;
-    // layout: [koff 16][six 4 pad 12][n_rec 4][need 4][pad 8][key ...][out ...]
-    u8* d_koff = d; u8* d_six = d + 16; u8* d_nrec = d + 32; u8* d_need = d + 36;
-    u8* d_key = d + 48; u8* d_out = d + 48 + align_up(klen, 16) + 16;
-    CUDA_OK(cudaMemcpyAsync(d_koff, koff, 16, cudaMemcpyHostToDevice, e->st));
-    CUDA_OK(cudaMemcpyAsync(d_six, &six, 4, cudaMemcpyHostToDevice, e->st));
-    if (klen) CUDA_OK(cudaMemcpyAsync(d_key, key, klen, cudaMemcpyHostToDevice, e->st));
-    VersionsArgs a{e->d_shards, d_view, (const u32*)d_six, d_key, (const u64*)d_koff, d_out, stride - 64, (u32*)d_nrec, (u32*)d_need, 1};
+    QLayout L;
+    const size_t o_koff = L.add(16), o_six = L.add(4), o_res = L.add(8), o_key = L.add(klen + 16), o_out = L.add(stride);
+    u8* d = (u8*)e->dev_q.get(L.size);
+    const u64 koff[2] = {0, klen};
+    const u32 six = s->index;
+    CUDA_OK(cudaMemcpyAsync(d + o_koff, koff, 16, cudaMemcpyHostToDevice, e->st));
+    CUDA_OK(cudaMemcpyAsync(d + o_six, &six, 4, cudaMemcpyHostToDevice, e->st));
+    if (klen) CUDA_OK(cudaMemcpyAsync(d + o_key, key, klen, cudaMemcpyHostToDevice, e->st));
+    u32* d_res = (u32*)(d + o_res);  // [n_rec, need]
+    VersionsArgs a{e->d_shards, d_view, (const u32*)(d + o_six), d + o_key, (const u64*)(d + o_koff), d + o_out, stride - 64, d_res, d_res + 1, 1};
     launch_get_versions(a, e->st);
     e->launches++;
     u32 res[2];
-    CUDA_OK(cudaMemcpyAsync(res, d_nrec, 8, cudaMemcpyDeviceToHost, e->st));
+    CUDA_OK(cudaMemcpyAsync(res, d_res, 8, cudaMemcpyDeviceToHost, e->st));
     CUDA_OK(cudaStreamSynchronize(e->st));
     if (res[1] > stride - 64) { stride = (size_t)res[1] * 2 + 128; continue; }
     std::vector<u8> buf(res[1] ? res[1] : 1);
-    if (res[1]) CUDA_OK(cudaMemcpy(buf.data(), d_out, res[1], cudaMemcpyDeviceToHost));
+    if (res[1]) CUDA_OK(cudaMemcpy(buf.data(), d + o_out, res[1], cudaMemcpyDeviceToHost));
     // records newest -> oldest; fold oldest -> newest
     struct Rec { u32 type; std::string v; };
     std::vector<Rec> recs;
@@ -1466,11 +1473,10 @@ static int multi_get_locked(rsp_engine* e, size_t n, const uint32_t* shard_ix, c
                             uint32_t klen_fixed, uint8_t* vals, size_t val_stride, uint32_t* vlen, int32_t* st) {
   if (n == 0) return RSP_OK;
   const size_t key_bytes = klen_fixed ? n * klen_fixed : (size_t)koff[n];
-  const size_t o_six = 0, o_koff = align_up(n * 4, 256), o_keys = o_koff + (klen_fixed ? 0 : align_up((n + 1) * 8, 256));
-  const size_t o_vlen = o_keys + align_up(key_bytes + 16, 256), o_st = o_vlen + align_up(n * 4, 256);
-  const size_t o_vals = o_st + align_up(n * 4, 256);
-  const size_t total = o_vals + n * val_stride + 256;
-  u8* d = (u8*)e->dev_q.get(total);
+  QLayout L;
+  const size_t o_six = L.add(n * 4), o_koff = L.add(klen_fixed ? 0 : (n + 1) * 8), o_keys = L.add(key_bytes + 16);
+  const size_t o_vlen = L.add(n * 4), o_st = L.add(n * 4), o_vals = L.add(n * val_stride + 256);
+  u8* d = (u8*)e->dev_q.get(L.size);
   const size_t CH = 1u << 18;
   const bool piped = klen_fixed && n >= 2 * CH;
   const size_t n_chunks = piped ? (n + CH - 1) / CH : 1;
@@ -1534,6 +1540,52 @@ static int multi_get_locked(rsp_engine* e, size_t n, const uint32_t* shard_ix, c
   return RSP_OK;
 }
 
+// One host-form launch of k_multi_scan (engine mutex held): `a` holds what the scans read, their flags and sizes;
+// shard_ix (or the table slots), keys and ends (nullptr: none) are host arrays, uploaded to dev_q.  n_out, st and the
+// n * a.out_stride bytes of records come back in one round trip; ms != nullptr: the kernel's time.
+static void scan_round_trip(rsp_engine* e, ScanArgs a, bool reverse, bool cat, const u32* shard_ix, const u8* keys,
+                            const u64* koff, const u8* ends, const u64* eoff, u8* out, u32* n_out, i32* st,
+                            float* ms) {
+  const size_t n = a.n, key_bytes = (size_t)koff[n], end_bytes = ends ? (size_t)eoff[n] : 0;
+  QLayout L;
+  const size_t o_six = L.add(n * 4), o_koff = L.add((n + 1) * 8), o_keys = L.add(key_bytes + 16);
+  const size_t o_eoff = L.add(ends ? (n + 1) * 8 : 0), o_ends = L.add(ends ? end_bytes + 16 : 0);
+  const size_t o_nout = L.add(n * 4), o_st = L.add(n * 4), o_out = L.add(n * a.out_stride + 256);
+  u8* d = (u8*)e->dev_q.get(L.size);
+  CUDA_OK(cudaMemcpyAsync(d + o_six, shard_ix, n * 4, cudaMemcpyHostToDevice, e->st));
+  CUDA_OK(cudaMemcpyAsync(d + o_koff, koff, (n + 1) * 8, cudaMemcpyHostToDevice, e->st));
+  if (key_bytes) CUDA_OK(cudaMemcpyAsync(d + o_keys, keys, key_bytes, cudaMemcpyHostToDevice, e->st));
+  a.shard_ix = (const u32*)(d + o_six); a.keys = d + o_keys; a.koff = (const u64*)(d + o_koff); a.klen_fixed = 0;
+  a.out = d + o_out; a.n_out = (u32*)(d + o_nout); a.st = (i32*)(d + o_st);
+  if (ends) {
+    CUDA_OK(cudaMemcpyAsync(d + o_eoff, eoff, (n + 1) * 8, cudaMemcpyHostToDevice, e->st));
+    if (end_bytes) CUDA_OK(cudaMemcpyAsync(d + o_ends, ends, end_bytes, cudaMemcpyHostToDevice, e->st));
+    a.ends = d + o_ends; a.eoff = (const u64*)(d + o_eoff);
+  }
+  if (ms) CUDA_OK(cudaEventRecord(e->ev0, e->st));
+  launch_multi_scan(a, reverse, cat, e->st);
+  e->launches++;
+  if (ms) CUDA_OK(cudaEventRecord(e->ev1, e->st));
+  CUDA_OK(cudaMemcpyAsync(n_out, d + o_nout, n * 4, cudaMemcpyDeviceToHost, e->st));
+  CUDA_OK(cudaMemcpyAsync(st, d + o_st, n * 4, cudaMemcpyDeviceToHost, e->st));
+  CUDA_OK(cudaMemcpyAsync(out, d + o_out, n * a.out_stride, cudaMemcpyDeviceToHost, e->st));
+  CUDA_OK(cudaStreamSynchronize(e->st));
+  if (ms) cudaEventElapsedTime(ms, e->ev0, e->ev1);
+}
+
+// f(rec, klen, vlen) for each of the n_out records [u32 klen][u32 vlen][key][value] of one scan (f may rewrite vlen);
+// a vlen marker (SCAN_VLEN_HOST_FOLD, SCAN_VLEN_MERGE_FAILED) has no value bytes
+template <class F>
+static void walk_scan_records(u8* rec, u32 n_out, F f) {
+  for (u32 i = 0; i < n_out; i++) {
+    u32 kl, vl;
+    memcpy(&kl, rec, 4);
+    memcpy(&vl, rec + 4, 4);
+    f(rec, kl, vl);
+    rec += 8 + kl + (vl == SCAN_VLEN_HOST_FOLD || vl == SCAN_VLEN_MERGE_FAILED ? 0 : vl);
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // iterator
 // ------------------------------------------------------------------------------------------------
@@ -1570,60 +1622,38 @@ static void iter_fetch(rsp_iter* it, const std::string* key, bool exclusive, boo
   it->reverse = reverse;
   std::string fetch_key;
   const bool bounded = it->has_upper && !reverse;
-  const size_t elen = bounded ? it->upper.size() : 0;
+  const u64 eoff[2] = {0, bounded ? it->upper.size() : 0};
+  const u32 slot = 0;  // the iterator's view is a one-entry snapshot table
   for (;;) {
-    const size_t klen = key ? key->size() : 0;
-    const size_t o_key = 64, o_ekey = 64 + align_up(klen + 16, 256), o_out = o_ekey + align_up(elen + 16, 256);
-    u8* d = (u8*)e->dev_q.get(o_out + it->stride + 256);
-    // header: [koff 2x8][pad][n_out 4 @32][st 4 @36][pad][eoff 2x8 @40]
-    u64 koff[2] = {0, klen};
-    CUDA_OK(cudaMemcpyAsync(d, koff, 16, cudaMemcpyHostToDevice, e->st));
-    if (klen) CUDA_OK(cudaMemcpyAsync(d + o_key, key->data(), klen, cudaMemcpyHostToDevice, e->st));
+    const u64 koff[2] = {0, key ? key->size() : 0};
     ScanArgs a;
-    a.shards = nullptr; a.views = it->d_view; a.shard_ix = nullptr; a.keys = d + o_key; a.koff = (const u64*)d;
-    a.klen_fixed = 0; a.flags = (exclusive ? SCAN_EXCLUSIVE : 0u) | (key ? 0u : SCAN_FROM_EXTREME);
-    a.max_entries = (u32)it->want; a.out = d + o_out; a.out_stride = it->stride;
-    a.n_out = (u32*)(d + 32); a.st = (i32*)(d + 36); a.n = 1;
-    if (bounded) {
-      const u64 eoff[2] = {0, elen};
-      CUDA_OK(cudaMemcpyAsync(d + 40, eoff, 16, cudaMemcpyHostToDevice, e->st));
-      if (elen) CUDA_OK(cudaMemcpyAsync(d + o_ekey, it->upper.data(), elen, cudaMemcpyHostToDevice, e->st));
-      a.ends = d + o_ekey; a.eoff = (const u64*)(d + 40);
-    }
-    launch_multi_scan(a, reverse, it->s->opts.merge_op == RSP_MERGE_STRING_APPEND, e->st);
-    e->launches++;
-    u32 res[2];
-    CUDA_OK(cudaMemcpyAsync(res, d + 32, 8, cudaMemcpyDeviceToHost, e->st));
-    CUDA_OK(cudaStreamSynchronize(e->st));
-    const u32 n_out = res[0];
-    const bool truncated = (i32)res[1] == RSP_INCOMPLETE || ((i32)res[1] & SCAN_ST_TRUNCATED) != 0;
-    const i32 st = (i32)res[1] & ~SCAN_ST_TRUNCATED;
-    if (n_out == 0 && truncated) { it->stride *= 4; continue; }
+    a.shards = nullptr; a.views = it->d_view; a.n_views = 1;
+    a.flags = SCAN_AT_SLOT | (exclusive ? SCAN_EXCLUSIVE : 0u) | (key ? 0u : SCAN_FROM_EXTREME);
+    a.max_entries = (u32)it->want; a.out_stride = it->stride; a.n = 1;
     std::vector<u8> h(it->stride);
-    if (n_out) CUDA_OK(cudaMemcpy(h.data(), d + o_out, it->stride, cudaMemcpyDeviceToHost));
-    size_t at = 0;
+    u32 n_out; i32 st_word;
+    scan_round_trip(e, a, reverse, it->s->opts.merge_op == RSP_MERGE_STRING_APPEND, &slot,
+                    key ? (const u8*)key->data() : nullptr, koff, bounded ? (const u8*)it->upper.data() : nullptr,
+                    eoff, h.data(), &n_out, &st_word, nullptr);
+    const bool truncated = st_word == RSP_INCOMPLETE || (st_word & SCAN_ST_TRUNCATED) != 0;
+    const i32 st = st_word & ~SCAN_ST_TRUNCATED;
+    if (n_out == 0 && truncated) { it->stride *= 4; continue; }
     std::string last_key;
-    for (u32 i = 0; i < n_out; i++) {
-      u32 kl, vl;
-      memcpy(&kl, &h[at], 4);
-      memcpy(&vl, &h[at + 4], 4);
-      std::string k((const char*)&h[at + 8], kl);
+    walk_scan_records(h.data(), n_out, [&](u8* r, u32 kl, u32 vl) {
+      std::string k((const char*)r + 8, kl);
       last_key = k;
       if (vl == SCAN_VLEN_HOST_FOLD) {  // operator lives on the host: fold this key against the pinned view
+        // (the fold reuses the scan's device scratch: the records are already on the host, in `h`)
         std::string v;
         const int rc = host_fold_get(e, it->s, (const uint8_t*)k.data(), k.size(), &v, it->d_view);
         if (rc == RSP_OK) it->buf.push_back({std::move(k), std::move(v), 0});
         else if (rc != RSP_NOT_FOUND) it->buf.push_back({std::move(k), std::string(), rc});
-        at += 8 + kl;
-        // (the scan kernel's scratch was reused by the fold: the copy in `h` is what we keep reading)
       } else if (vl == SCAN_VLEN_MERGE_FAILED) {
         it->buf.push_back({std::move(k), std::string(), st > 255 ? (int)(st >> 8) : RSP_CORRUPTION});
-        at += 8 + kl;
       } else {
-        it->buf.push_back({std::move(k), std::string((const char*)&h[at + 8 + kl], vl), 0});
-        at += 8 + kl + vl;
+        it->buf.push_back({std::move(k), std::string((const char*)r + 8 + kl, vl), 0});
       }
-    }
+    });
     it->exhausted = !(truncated || n_out == it->want);
     if (g_trace) fprintf(stderr, "[rsp trace] iter_fetch want=%zu stride=%zu reverse=%d exclusive=%d klen=%zu -> n_out=%u st=%d kept=%zu exhausted=%d\n",
                          it->want, it->stride, (int)reverse, (int)exclusive, key ? key->size() : 0, n_out, st, it->buf.size(), (int)it->exhausted);
@@ -2743,39 +2773,34 @@ int rsp_get_stats(const rsp_shard* s, rsp_stats* out) {
 }
 
 // ---- iterator ----
-rsp_iter* rsp_iter_create(rsp_shard* s) {
-  try {
-  if (!s) return nullptr;
-  rsp_engine* e = s->eng;
-  std::lock_guard<std::mutex> g(e->mu);
-  if (ticks_in_flight(s)) return nullptr;  // fold the pre-staged ticks first (rsp_apply_staged_finish)
-  rsp_iter* it = new rsp_iter();
-  it->s = s;
-  CUDA_OK(cudaSetDevice(e->device));
-  ScanView v;
-  pin_view(e, s, &it->pinned, &v);
-  it->d_view = (ScanView*)e->arena.alloc(sizeof(ScanView));
-  CUDA_OK(cudaMemcpyAsync(it->d_view, &v, sizeof(v), cudaMemcpyHostToDevice, e->st));
-  CUDA_OK(cudaStreamSynchronize(e->st));
-  return it;
-  } catch (...) { abi_caught(); return nullptr; }
-}
-// an iterator over a snapshot's runs: it takes its own pins, so it may outlive the snapshot
-rsp_iter* rsp_iter_create_at(rsp_snapshot* snap) {
-  try {
-  if (!snap) return nullptr;
-  rsp_engine* e = snap->s->eng;
-  std::lock_guard<std::mutex> g(e->mu);
+// an iterator over the shard's current contents, or over a snapshot's runs (with its own pins: it may outlive the
+// snapshot); its view goes to the arena as a one-entry snapshot table, scanned at slot 0.  Engine mutex held.
+static rsp_iter* iter_new(rsp_engine* e, rsp_shard* s, const rsp_snapshot* snap) {
   CUDA_OK(cudaSetDevice(e->device));
   std::unique_ptr<rsp_iter> it(new rsp_iter());
-  it->s = snap->s;
-  it->pinned = snap->pinned;
+  it->s = s;
   ScanView v;
-  view_of(snap->s, it->pinned, &v);
+  if (snap) { it->pinned = snap->pinned; view_of(s, it->pinned, &v); }
+  else pin_view(e, s, &it->pinned, &v);
+  v.live = 1;
   it->d_view = (ScanView*)e->arena.alloc(sizeof(ScanView));
   CUDA_OK(cudaMemcpyAsync(it->d_view, &v, sizeof(v), cudaMemcpyHostToDevice, e->st));
   CUDA_OK(cudaStreamSynchronize(e->st));
   return it.release();
+}
+rsp_iter* rsp_iter_create(rsp_shard* s) {
+  try {
+  if (!s) return nullptr;
+  std::lock_guard<std::mutex> g(s->eng->mu);
+  if (ticks_in_flight(s)) return nullptr;  // fold the pre-staged ticks first (rsp_apply_staged_finish)
+  return iter_new(s->eng, s, nullptr);
+  } catch (...) { abi_caught(); return nullptr; }
+}
+rsp_iter* rsp_iter_create_at(rsp_snapshot* snap) {
+  try {
+  if (!snap) return nullptr;
+  std::lock_guard<std::mutex> g(snap->s->eng->mu);
+  return iter_new(snap->s->eng, snap->s, snap);
   } catch (...) { abi_caught(); return nullptr; }
 }
 void rsp_iter_destroy(rsp_iter* it) {
@@ -2922,24 +2947,31 @@ void rsp_snapshot_release(rsp_snapshot* snap) {
 uint64_t rsp_snapshot_seq(const rsp_snapshot* snap) { return snap ? snap->seq : 0; }
 uint32_t rsp_snapshot_slot(const rsp_snapshot* snap) { return snap ? snap->slot : 0xffffffffu; }
 
+// the snapshot table slot of each read; a NULL or foreign handle gets NO_SLOT: InvalidArgument for that read alone
+constexpr u32 NO_SLOT = 0xffffffffu;
+static std::vector<u32> snapshot_slots(const rsp_engine* e, size_t n, rsp_snapshot* const* snaps) {
+  std::vector<u32> slot(n);
+  for (size_t i = 0; i < n; i++) slot[i] = snaps[i] && snaps[i]->s->eng == e ? snaps[i]->slot : NO_SLOT;
+  return slot;
+}
+
 // MultiGet at snapshots over host buffers (engine mutex held): one launch of k_multi_get_at on the engine stream; the
 // rare statuses (host-folded merge operators, error texts) are finished on the host against the snapshot's view
 static int multi_get_at_locked(rsp_engine* e, size_t n, rsp_snapshot* const* snaps, const uint8_t* keys,
                                const uint64_t* koff, uint8_t* vals, size_t val_stride, uint32_t* vlen, int32_t* st) {
   if (n == 0) return RSP_OK;
-  std::vector<u32> slot(n);
-  for (size_t i = 0; i < n; i++) slot[i] = snaps[i] && snaps[i]->s->eng == e ? snaps[i]->slot : 0xffffffffu;
+  const std::vector<u32> slot = snapshot_slots(e, n, snaps);
   const size_t key_bytes = (size_t)koff[n];
-  const size_t o_koff = align_up(n * 4, 256), o_keys = o_koff + align_up((n + 1) * 8, 256);
-  const size_t o_vlen = o_keys + align_up(key_bytes + 16, 256), o_st = o_vlen + align_up(n * 4, 256);
-  const size_t o_spec = o_st + align_up(n * 4, 256), o_vals = o_spec + 256;
-  u8* d = (u8*)e->dev_q.get(o_vals + n * val_stride + 256);
-  CUDA_OK(cudaMemcpyAsync(d, slot.data(), n * 4, cudaMemcpyHostToDevice, e->st));
+  QLayout L;
+  const size_t o_slot = L.add(n * 4), o_koff = L.add((n + 1) * 8), o_keys = L.add(key_bytes + 16);
+  const size_t o_vlen = L.add(n * 4), o_st = L.add(n * 4), o_spec = L.add(4), o_vals = L.add(n * val_stride + 256);
+  u8* d = (u8*)e->dev_q.get(L.size);
+  CUDA_OK(cudaMemcpyAsync(d + o_slot, slot.data(), n * 4, cudaMemcpyHostToDevice, e->st));
   CUDA_OK(cudaMemcpyAsync(d + o_koff, koff, (n + 1) * 8, cudaMemcpyHostToDevice, e->st));
   if (key_bytes) CUDA_OK(cudaMemcpyAsync(d + o_keys, keys, key_bytes, cudaMemcpyHostToDevice, e->st));
   CUDA_OK(cudaMemsetAsync(d + o_spec, 0, 4, e->st));
   GetAtArgs a;
-  a.views = e->d_snap_views; a.slot = (const u32*)d; a.keys = d + o_keys; a.koff = (const u64*)(d + o_koff);
+  a.views = e->d_snap_views; a.slot = (const u32*)(d + o_slot); a.keys = d + o_keys; a.koff = (const u64*)(d + o_koff);
   a.vals = d + o_vals; a.val_stride = val_stride; a.vlen = (u32*)(d + o_vlen); a.st = (i32*)(d + o_st);
   a.n_special = (u32*)(d + o_spec); a.n_views = e->d_snap_views ? RSP_MAX_SNAPSHOTS : 0; a.klen_fixed = 0; a.n = (u32)n;
   CUDA_OK(cudaEventRecord(e->ev0, e->st));
@@ -2958,7 +2990,7 @@ static int multi_get_at_locked(rsp_engine* e, size_t n, rsp_snapshot* const* sna
   e->last_ms["multi_get_at"] = ms;
   if (!n_special) return RSP_OK;
   finish_special(e, n, [&](size_t i) {
-    if (slot[i] == 0xffffffffu) return LookupRef{nullptr, nullptr, 0, nullptr};  // InvalidArgument, no text
+    if (slot[i] == NO_SLOT) return LookupRef{nullptr, nullptr, 0, nullptr};  // InvalidArgument, no text
     return LookupRef{snaps[i]->s, keys + koff[i], (size_t)(koff[i + 1] - koff[i]), e->d_snap_views + slot[i]};
   }, vals, val_stride, vlen, st);
   return RSP_OK;
@@ -3031,9 +3063,7 @@ static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, rs
   if (n == 0) return RSP_OK;
   std::vector<u32> slot;
   if (at) {
-    // a NULL or foreign handle gets a slot the kernel refuses: InvalidArgument for that scan alone
-    slot.resize(n);
-    for (size_t i = 0; i < n; i++) slot[i] = snaps[i] && snaps[i]->s->eng == e ? snaps[i]->slot : 0xffffffffu;
+    slot = snapshot_slots(e, n, snaps);
     shard_ix = slot.data();
   } else {
     std::vector<rsp_shard*> fl;
@@ -3047,38 +3077,12 @@ static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, rs
   }
   std::vector<uint64_t> no_keys;
   if (from_extreme) { no_keys.assign(n + 1, 0); koff = no_keys.data(); }
-  const size_t key_bytes = (size_t)koff[n], end_bytes = ends ? (size_t)eoff[n] : 0;
-  const size_t o_koff = align_up(n * 4, 256), o_keys = o_koff + align_up((n + 1) * 8, 256);
-  const size_t o_eoff = o_keys + align_up(key_bytes + 16, 256), o_ends = o_eoff + (ends ? align_up((n + 1) * 8, 256) : 0);
-  const size_t o_nout = o_ends + (ends ? align_up(end_bytes + 16, 256) : 0), o_st = o_nout + align_up(n * 4, 256);
-  const size_t o_out = o_st + align_up(n * 4, 256);
-  u8* d = (u8*)e->dev_q.get(o_out + n * out_stride + 256);
-  CUDA_OK(cudaMemcpyAsync(d, shard_ix, n * 4, cudaMemcpyHostToDevice, e->st));
-  CUDA_OK(cudaMemcpyAsync(d + o_koff, koff, (n + 1) * 8, cudaMemcpyHostToDevice, e->st));
-  if (key_bytes) CUDA_OK(cudaMemcpyAsync(d + o_keys, keys, key_bytes, cudaMemcpyHostToDevice, e->st));
   ScanArgs a;
-  a.shards = e->d_shards; a.views = nullptr; a.shard_ix = (const u32*)d; a.keys = d + o_keys;
-  a.koff = (const u64*)(d + o_koff); a.klen_fixed = 0; a.max_entries = max_entries;
-  a.flags = (exclusive ? SCAN_EXCLUSIVE : 0u) | (from_extreme ? SCAN_FROM_EXTREME : 0u);
-  if (at) {
-    a.views = e->d_snap_views; a.n_views = e->d_snap_views ? RSP_MAX_SNAPSHOTS : 0; a.flags |= SCAN_AT_SLOT;
-  }
-  a.out = d + o_out; a.out_stride = out_stride; a.n_out = (u32*)(d + o_nout); a.st = (i32*)(d + o_st); a.n = (u32)n;
-  if (ends) {
-    CUDA_OK(cudaMemcpyAsync(d + o_eoff, eoff, (n + 1) * 8, cudaMemcpyHostToDevice, e->st));
-    if (end_bytes) CUDA_OK(cudaMemcpyAsync(d + o_ends, ends, end_bytes, cudaMemcpyHostToDevice, e->st));
-    a.ends = d + o_ends; a.eoff = (const u64*)(d + o_eoff);
-  }
-  CUDA_OK(cudaEventRecord(e->ev0, e->st));
-  launch_multi_scan(a, reverse, cat_reads(e), e->st);
-  e->launches++;
-  CUDA_OK(cudaEventRecord(e->ev1, e->st));
-  CUDA_OK(cudaMemcpyAsync(n_out, d + o_nout, n * 4, cudaMemcpyDeviceToHost, e->st));
-  CUDA_OK(cudaMemcpyAsync(st, d + o_st, n * 4, cudaMemcpyDeviceToHost, e->st));
-  CUDA_OK(cudaMemcpyAsync(out, d + o_out, n * out_stride, cudaMemcpyDeviceToHost, e->st));
-  CUDA_OK(cudaStreamSynchronize(e->st));
+  a.shards = e->d_shards; a.views = at ? e->d_snap_views : nullptr; a.n_views = a.views ? RSP_MAX_SNAPSHOTS : 0;
+  a.flags =(exclusive ? SCAN_EXCLUSIVE : 0u) | (from_extreme ? SCAN_FROM_EXTREME : 0u) | (at ? SCAN_AT_SLOT : 0u);
+  a.max_entries = max_entries; a.out_stride = out_stride; a.n = (u32)n;
   float ms = 0;
-  cudaEventElapsedTime(&ms, e->ev0, e->ev1);
+  scan_round_trip(e, a, reverse, cat_reads(e), shard_ix, keys, koff, ends, eoff, out, n_out, st, &ms);
   e->last_ms["scan"] = ms;
   for (size_t i = 0; i < n; i++) {
     st[i] &= ~SCAN_ST_TRUNCATED;  // (n_out[i] < max_entries tells the caller that the scan stopped early)
@@ -3086,14 +3090,9 @@ static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, rs
     else if (st[i] > 255) {
       // a merge failed somewhere in this scan: its record reads as an empty value, the status is the scan's
       st[i] = st[i] >> 8;
-      u8* r = out + i * out_stride;
-      for (u32 k = 0; k < n_out[i]; k++) {
-        u32 kl, vl;
-        memcpy(&kl, r, 4);
-        memcpy(&vl, r + 4, 4);
-        if (vl == SCAN_VLEN_MERGE_FAILED) { vl = 0; memcpy(r + 4, &vl, 4); }
-        r += 8 + kl + vl;
-      }
+      walk_scan_records(out + i * out_stride, n_out[i], [](u8* r, u32, u32 vl) {
+        if (vl == SCAN_VLEN_MERGE_FAILED) memset(r + 4, 0, 4);
+      });
     }
   }
   return RSP_OK;

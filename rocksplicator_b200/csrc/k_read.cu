@@ -871,20 +871,16 @@ __device__ __forceinline__ void multi_scan_body(const ScanArgs& a) {
   if (q >= a.n) return;
   const RunDev* runs;
   u32 n_runs, merge_op, merge_delim = 0;
-  // SCAN_AT_SLOT is tested first: without a snapshot table (views == nullptr, n_views == 0) every slot is refused here
-  // instead of being read as a shard index
-  const ScanView* vw = a.views + q;
   if (a.flags & SCAN_AT_SLOT) {
+    // without a snapshot table (views == nullptr, n_views == 0) every slot is refused
     const u32 slot = a.shard_ix[q];
     if (slot >= a.n_views || !a.views[slot].live) {
       if (lane == 0) { a.n_out[q] = 0; a.st[q] = 4; }  // InvalidArgument, as k_multi_get_at
       return;
     }
-    vw = a.views + slot;
-  }
-  if (a.views) {
-    runs = vw->runs; n_runs = vw->n_runs; merge_op = vw->merge_op;
-    if constexpr (CAT) merge_delim = vw->merge_delim;
+    const ScanView& vw = a.views[slot];
+    runs = vw.runs; n_runs = vw.n_runs; merge_op = vw.merge_op;
+    if constexpr (CAT) merge_delim = vw.merge_delim;
   } else {
     const ShardDev* sd = a.shards + a.shard_ix[q];
     runs = sd->runs; n_runs = sd->n_runs; merge_op = sd->merge_op;

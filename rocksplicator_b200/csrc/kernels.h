@@ -185,8 +185,8 @@ constexpr u32 SCAN_VLEN_MERGE_FAILED = 0xfffffffeu;  // the merge failed: empty 
 // mk_status(code, msg) of a failed merge; the last two carry SCAN_ST_TRUNCATED when the scan ALSO ran out of room
 constexpr i32 SCAN_ST_TRUNCATED = 1 << 30;
 struct ScanArgs {
-  const ShardDev* shards;   // used when views == nullptr (shard_ix indexes it)
-  const ScanView* views;    // or explicit pinned views: one per request, or the snapshot table (SCAN_AT_SLOT)
+  const ShardDev* shards;   // without SCAN_AT_SLOT: shard_ix indexes it
+  const ScanView* views;    // SCAN_AT_SLOT: the snapshot table (an iterator's own view is a one-entry table)
   const u32* shard_ix;      // (SCAN_AT_SLOT: the snapshot table slot of each request)
   const u8* keys;
   const u64* koff;

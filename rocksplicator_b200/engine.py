@@ -175,6 +175,11 @@ def _pack_keys(keys):
     return np.frombuffer(b"".join(keys) + b"\0", dtype=np.uint8), off
 
 
+def _handles(snapshots):
+    """Snapshots (or None) -> the C array of their handles"""
+    return (C.c_void_p * max(len(snapshots), 1))(*[s.h if s is not None else None for s in snapshots])
+
+
 def _scan_records(out, n_out, st, n, stride):
     """the [u32 klen][u32 vlen][key][value] records of n scans at out + i * stride -> [(status, [(key, value)])].  A key
     that needs a host-side merge operator (RSP_MERGE_APPEND or RSP_MERGE_CALLBACK: vlen 0xffffffff, no value bytes; the
@@ -497,78 +502,56 @@ class Engine:
         return self.lib.rsp_multi_get_fixed(self.h, len(six), _ptr(six), _ptr(keys), klen, _ptr(vals), stride,
                                             _ptr(vlen), _ptr(st))
 
-    def multi_scan(self, shard_ix, keys, max_entries, stride, ends=None):
-        """scan i: up to max_entries live entries from keys[i], before ends[i] (exclusive) when ends is given ->
-        [(status, [(key, value)])]"""
-        n = len(keys)
-        six = np.ascontiguousarray(shard_ix, dtype=np.uint32)
-        blob, off = _pack_keys(keys)
-        out = np.zeros(max(n * stride, 1), dtype=np.uint8)
-        n_out = np.zeros(max(n, 1), dtype=np.uint32)
-        st = np.zeros(max(n, 1), dtype=np.int32)
-        if ends is None:
-            rc = self.lib.rsp_multi_scan(self.h, n, _ptr(six), _ptr(blob), _ptr(off), max_entries, _ptr(out), stride,
-                                         _ptr(n_out), _ptr(st))
-        else:
-            if len(ends) != n:
-                raise ValueError("one end key per scan")
-            eblob, eoff = _pack_keys(ends)
-            rc = self.lib.rsp_multi_scan_bounded(self.h, n, _ptr(six), _ptr(blob), _ptr(off), _ptr(eblob), _ptr(eoff),
-                                                 max_entries, _ptr(out), stride, _ptr(n_out), _ptr(st))
-        if rc != OK:
-            raise RuntimeError(f"rsp_multi_scan -> {rc}")
-        return _scan_records(out, n_out, st, n, stride)
-
-    def multi_scan_reverse(self, shard_ix, keys, max_entries, stride, lows=None, exclusive=False):
-        """reverse scan i (SeekForPrev + Prev): up to max_entries live entries in descending key order from the last key
-        <= keys[i] (< keys[i] when exclusive; keys=None: from the shard's last key), down to lows[i] (inclusive) when
-        lows is given -> [(status, [(key, value)])].  [a, b) newest-first: keys=[b], lows=[a], exclusive=True."""
-        n = len(shard_ix)
-        six = np.ascontiguousarray(shard_ix, dtype=np.uint32)
-        if keys is not None and len(keys) != n:
-            raise ValueError("one start key per scan")
-        if lows is not None and len(lows) != n:
-            raise ValueError("one low key per scan")
-        blob, off = _pack_keys(keys) if keys is not None else (None, None)
-        lblob, loff = _pack_keys(lows) if lows is not None else (None, None)
-        out = np.zeros(max(n * stride, 1), dtype=np.uint8)
-        n_out = np.zeros(max(n, 1), dtype=np.uint32)
-        st = np.zeros(max(n, 1), dtype=np.int32)
-        rc = self.lib.rsp_multi_scan_reverse(self.h, n, _ptr(six), _ptr(blob), _ptr(off), 1 if exclusive else 0,
-                                             _ptr(lblob), _ptr(loff), max_entries, _ptr(out), stride, _ptr(n_out),
-                                             _ptr(st))
-        if rc != OK:
-            raise RuntimeError(f"rsp_multi_scan_reverse -> {rc}")
-        return _scan_records(out, n_out, st, n, stride)
-
-    def _scan_at(self, fn, snapshots, keys, max_entries, stride, ends, exclusive):
-        n = len(snapshots)
+    def _scan(self, fn, n, first, keys, ends, max_entries, stride, exclusive=None, ends_are="end"):
+        """one call of the host-form scan entry point `fn`: `first` is the shard indices or the snapshot handles, keys
+        and ends are byte strings (None: none) -> [(status, [(key, value)])].  exclusive=None: `fn` takes no exclusive
+        flag (rsp_multi_scan, rsp_multi_scan_bounded); rsp_multi_scan alone takes no end keys."""
         if keys is not None and len(keys) != n:
             raise ValueError("one start key per scan")
         if ends is not None and len(ends) != n:
-            raise ValueError("one end key per scan")
-        handles = (C.c_void_p * max(n, 1))(*[s.h if s is not None else None for s in snapshots])
+            raise ValueError(f"one {ends_are} key per scan")
         blob, off = _pack_keys(keys) if keys is not None else (None, None)
         eblob, eoff = _pack_keys(ends) if ends is not None else (None, None)
         out = np.zeros(max(n * stride, 1), dtype=np.uint8)
         n_out = np.zeros(max(n, 1), dtype=np.uint32)
         st = np.zeros(max(n, 1), dtype=np.int32)
-        rc = getattr(self.lib, fn)(self.h, n, handles, _ptr(blob), _ptr(off), 1 if exclusive else 0, _ptr(eblob),
-                                   _ptr(eoff), max_entries, _ptr(out), stride, _ptr(n_out), _ptr(st))
+        args = [self.h, n, first, _ptr(blob), _ptr(off)]
+        if exclusive is not None:
+            args.append(1 if exclusive else 0)
+        if fn != "rsp_multi_scan":
+            args += [_ptr(eblob), _ptr(eoff)]
+        rc = getattr(self.lib, fn)(*args, max_entries, _ptr(out), stride, _ptr(n_out), _ptr(st))
         if rc != OK:
             raise RuntimeError(f"{fn} -> {rc}")
         return _scan_records(out, n_out, st, n, stride)
+
+    def multi_scan(self, shard_ix, keys, max_entries, stride, ends=None):
+        """scan i: up to max_entries live entries from keys[i], before ends[i] (exclusive) when ends is given ->
+        [(status, [(key, value)])]"""
+        six = np.ascontiguousarray(shard_ix, dtype=np.uint32)
+        fn = "rsp_multi_scan" if ends is None else "rsp_multi_scan_bounded"
+        return self._scan(fn, len(keys), _ptr(six), keys, ends, max_entries, stride)
+
+    def multi_scan_reverse(self, shard_ix, keys, max_entries, stride, lows=None, exclusive=False):
+        """reverse scan i (SeekForPrev + Prev): up to max_entries live entries in descending key order from the last key
+        <= keys[i] (< keys[i] when exclusive; keys=None: from the shard's last key), down to lows[i] (inclusive) when
+        lows is given -> [(status, [(key, value)])].  [a, b) newest-first: keys=[b], lows=[a], exclusive=True."""
+        six = np.ascontiguousarray(shard_ix, dtype=np.uint32)
+        return self._scan("rsp_multi_scan_reverse", len(six), _ptr(six), keys, lows, max_entries, stride, exclusive,
+                          ends_are="low")
 
     def multi_scan_at(self, snapshots, keys, max_entries, stride, ends=None, exclusive=False):
         """scan i at snapshots[i] (a Snapshot, or None: InvalidArgument): up to max_entries live entries from keys[i]
         (after it when exclusive; keys=None: from the snapshot's first key), before ends[i] (exclusive) when ends is
         given -> [(status, [(key, value)])].  Flushes nothing."""
-        return self._scan_at("rsp_multi_scan_at", snapshots, keys, max_entries, stride, ends, exclusive)
+        return self._scan("rsp_multi_scan_at", len(snapshots), _handles(snapshots), keys, ends, max_entries, stride,
+                          exclusive)
 
     def multi_scan_reverse_at(self, snapshots, keys, max_entries, stride, lows=None, exclusive=False):
         """multi_scan_reverse at snapshots[i] (keys=None: from the snapshot's last key) -> [(status, [(key, value)])].
         Flushes nothing."""
-        return self._scan_at("rsp_multi_scan_reverse_at", snapshots, keys, max_entries, stride, lows, exclusive)
+        return self._scan("rsp_multi_scan_reverse_at", len(snapshots), _handles(snapshots), keys, lows, max_entries,
+                          stride, exclusive)
 
     def flush_all(self): return self.lib.rsp_flush_all(self.h)
     def compact_all(self): return self.lib.rsp_compact_all(self.h)
