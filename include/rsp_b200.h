@@ -105,6 +105,12 @@ int rsp_engine_device(const rsp_engine* e);
 /* the engine's CUDA stream (cudaStream_t as void*): lets a caller order its own work / events with it */
 void* rsp_engine_stream(const rsp_engine* e);
 int rsp_shard_open(rsp_engine* e, const char* name, const rsp_shard_opts* opts, rsp_shard** out);
+/* rsp_shard_open with RSP_SHARD_* flags (rsp_shard_open is flags 0; an unknown flag answers InvalidArgument).
+ * RSP_SHARD_ALLOW_INGEST_BEHIND == DBOptions::allow_ingest_behind: the shard keeps a bottom tier for files ingested
+ * behind its data (rsp_ingest_sorted_behind), and so no flush or compaction counts as bottom-most: tombstones are kept,
+ * and merge operands with no base below them stay operands. */
+#define RSP_SHARD_ALLOW_INGEST_BEHIND 1u
+int rsp_shard_open_ex(rsp_engine* e, const char* name, const rsp_shard_opts* opts, uint32_t flags, rsp_shard** out);
 int rsp_shard_close(rsp_shard* s); /* frees the shard's HBM (removeDB + DB close); the caller drains its own calls on
                                      * the shard first, as RocksDBReplicator::removeDB does (rocksdb_replicator.cpp:143-151) */
 uint32_t rsp_shard_index(const rsp_shard* s); /* index used by the batched calls below */
@@ -292,6 +298,11 @@ int rsp_multi_scan_reverse_at(rsp_engine* e, size_t n, rsp_snapshot* const* snap
  * (application_db.cpp:138-144; triggers admin_handler.cpp:1846,2174) -------------------------------- */
 int rsp_flush(rsp_shard* s);
 int rsp_compact(rsp_shard* s);
+/* rsp_compact with RSP_COMPACT_* flags (rsp_compact is flags 0).  rsp_compact leaves the ingested-behind tier alone
+ * (CompactRange with change_level = false); RSP_COMPACT_CHANGE_LEVEL (change_level = true) folds it in as well, and the
+ * shard's data becomes one ordinary run: the tier is empty afterwards. */
+#define RSP_COMPACT_CHANGE_LEVEL 1u
+int rsp_compact_ex(rsp_shard* s, uint32_t flags);
 int rsp_flush_all(rsp_engine* e);
 int rsp_compact_all(rsp_engine* e);
 int rsp_get_stats(const rsp_shard* s, rsp_stats* out);
@@ -303,6 +314,25 @@ int rsp_get_stats(const rsp_shard* s, rsp_stats* out);
  * InvalidArgument unless allow_global_seqno.  host/sst/sst_format.h turns an SST file into these arrays. */
 int rsp_ingest_sorted(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_t* koff, const uint8_t* vals,
                       const uint64_t* voff, int allow_global_seqno, uint64_t* seq_out);
+/* IngestExternalFileOptions::ingest_behind (RocksDB 5.7): the same input becomes a run of the shard's ingested-behind
+ * tier, below everything the shard holds.  Every earlier and later write to a key shadows the file's value, deletes
+ * hide it, merge operands fold onto it.  The sequence number does not move and the memtable is not flushed.  Iterators
+ * created before the call keep their own view and do not see the file.  Refusals change nothing and set
+ * rsp_last_error:
+ *   InvalidArgument "can't ingest_behind file in DB with allow_ingest_behind=false": the shard was opened without
+ *     RSP_SHARD_ALLOW_INGEST_BEHIND;
+ *   InvalidArgument "Can't ingest_behind file as it doesn't fit at the bottommost level!": the key range overlaps a
+ *     file already ingested behind;
+ *   InvalidArgument "Can't ingest_behind file as despite allow_ingest_behind=true there are files with 0 seqno in
+ *     database at upper levels!": an rsp_ingest_sorted file that took no global sequence number, or the result of an
+ *     RSP_COMPACT_CHANGE_LEVEL compaction that absorbed the tier, is still above it;
+ *   NotSupported while the shard has live snapshots (RocksDB would show the file to them; a snapshot's view is fixed).
+ * Flushes, background merges and rsp_compact never take the tier's runs as inputs; when the run table would overflow
+ * the tier's runs (key-disjoint, all at sequence 0) are merged with each other.  They count in rsp_stats.n_runs. */
+int rsp_ingest_sorted_behind(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_t* koff, const uint8_t* vals,
+                             const uint64_t* voff);
+/* bytes held by the ingested-behind tier (the bottom level of GetColumnFamilyMetaData); 0 = the tier is empty */
+uint64_t rsp_shard_behind_bytes(const rsp_shard* s);
 
 /* ---- device-pointer forms (kernel-level measurement; inputs/outputs already in HBM) -------------
  * `stream` is a cudaStream_t passed as void* (0 = the engine's own read stream).  No host

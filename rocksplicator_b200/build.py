@@ -70,12 +70,13 @@ HOST_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "host_tests")
 SNAPSHOT_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "snapshot_tests")
 BOUNDED_ITER_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "bounded_iter_tests")
 STRING_APPEND_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "string_append_tests")
+INGEST_BEHIND_TESTS = os.path.join(os.path.dirname(HERE), "tests", "cpp", "ingest_behind_tests")
 
 
 def build_host(force=False, verbose=False):
     """The C++ mirror of the reference interfaces (host/) -> librsp_host.so, and its test binaries (snapshot_tests,
-    bounded_iter_tests and string_append_tests are returned by build_snapshot_tests, build_bounded_iter_tests and
-    build_string_append_tests)."""
+    bounded_iter_tests, string_append_tests and ingest_behind_tests are returned by build_snapshot_tests,
+    build_bounded_iter_tests, build_string_append_tests and build_ingest_behind_tests)."""
     build(force=False, verbose=verbose)
     srcs = [os.path.join(HOST, s) for s in HOST_SRCS]
     deps = list(srcs)
@@ -95,7 +96,7 @@ def build_host(force=False, verbose=False):
     if force or _stale(HOST_TESTS, [tsrc, HOST_SO] + deps):
         run([cxx] + flags + ["-o", HOST_TESTS, tsrc, "-L", HERE, "-lrsp_host", "-lrsp_b200",
                              "-Wl,-rpath," + HERE])
-    for exe in (SNAPSHOT_TESTS, BOUNDED_ITER_TESTS, STRING_APPEND_TESTS):
+    for exe in (SNAPSHOT_TESTS, BOUNDED_ITER_TESTS, STRING_APPEND_TESTS, INGEST_BEHIND_TESTS):
         src = exe + ".cpp"
         if force or _stale(exe, [src, HOST_SO] + deps):
             run([cxx] + flags + ["-o", exe, src, "-L", HERE, "-lrsp_host", "-lrsp_b200", "-Wl,-rpath," + HERE])
@@ -120,3 +121,10 @@ def build_string_append_tests(force=False, verbose=False):
     reads at snapshots, Backup / Restore)"""
     build_host(force=force, verbose=verbose)
     return STRING_APPEND_TESTS
+
+
+def build_ingest_behind_tests(force=False, verbose=False):
+    """tests/cpp/ingest_behind_tests: Options::allow_ingest_behind, IngestExternalFileOptions::ingest_behind and
+    CompactRange(change_level) through GpuDB / ApplicationDB (application_db_test.cpp:300-342 step for step)"""
+    build_host(force=force, verbose=verbose)
+    return INGEST_BEHIND_TESTS

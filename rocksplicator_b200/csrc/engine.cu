@@ -142,6 +142,13 @@ struct Run {
   u32* hslots = nullptr;
   u64* blk_pfx = nullptr;
   u32 n_ent = 0, heap_units = 0, n_buckets = 0, ord_bits = 0, uniform_units = 0, n_blocks = 0, flags = 0, kv_len = 0;
+  // host-only: behind = the run belongs to the ingested-behind tier of an allow-ingest-behind shard (the oldest runs,
+  // key-disjoint, all at sequence 0); seq0 = the run holds sequence-0 data (an ingest that took no global sequence
+  // number, or what a compaction made of such runs)
+  bool behind = false, seq0 = false;
+  // behind runs: the key range [first, last] of every file the run holds (RocksDB keeps them as separate files at the
+  // bottom level, so a later file may fit between two of them)
+  std::vector<std::pair<std::string, std::string>> file_ranges;
   RunDev dev() const {
     RunDev r;
     r.heap = heap; r.ent_off = ent_off; r.hslots = hslots; r.blk_pfx = blk_pfx;
@@ -181,7 +188,20 @@ struct rsp_shard {
   u64 uid = 0;                    // never reused: a background merge recognises the shard it planned for
   const Run* bg_first_pinned = nullptr;
   u32 n_snapshots = 0;            // live rsp_snapshot handles on this shard
+  u32 open_flags = 0;             // RSP_SHARD_* of rsp_shard_open_ex
 };
+
+// runs the ingested-behind tier may hold: a further file first merges the tier's runs into one.  The foreground merge
+// of a flush starts when the whole table is nearly full, tier included: a small tier keeps that as rare as it is on a
+// shard without one
+constexpr size_t BEHIND_MAX_RUNS = 2;
+
+// runs of the shard's ingested-behind tier: the oldest end of s->runs
+static size_t behind_runs(const rsp_shard* s) {
+  size_t k = 0;
+  while (k < s->runs.size() && s->runs[s->runs.size() - 1 - k]->behind) k++;
+  return k;
+}
 
 // DB::GetSnapshot: the shard's contents at one sequence number, as a pinned set of runs (the memtable's contents
 // sorted into a private run first).  Its ScanView sits in slot `slot` of the engine's snapshot table.
@@ -245,7 +265,7 @@ struct rsp_engine {
   ShardFast* d_fast = nullptr;
   std::vector<rsp_shard*> slots;
   std::unordered_map<std::string, rsp_shard*> by_name;
-  PinBuf pin_in, pin_out, pin_up, pin_totals;
+  PinBuf pin_in, pin_out, pin_up, pin_totals, pin_ingest;
   DevBuf dev_tick, dev_q, dev_pending, dev_up;
   cudaEvent_t pending_ev = nullptr;  // the last device-form MultiGet launch (the pending list is per engine)
   bool pending_ev_recorded = false;
@@ -427,8 +447,14 @@ enum CompactMode {
   COMPACT_FLUSH,     // memtable -> new run; the newest runs join only when the run table is nearly full
   COMPACT_FULL,      // everything into one run (CompactRange(nullptr, nullptr))
   COMPACT_SNAPSHOT,  // memtable -> a private sorted run for an iterator; the shard is left untouched
-  COMPACT_MERGE      // background: the size-tiered merge set of the runs, no memtable
+  COMPACT_MERGE,     // background: the size-tiered merge set of the runs, no memtable
+  COMPACT_LEVEL,     // everything, the ingested-behind tier included, into one ordinary run (CompactRange change_level)
+  COMPACT_BEHIND     // the ingested-behind tier into one behind run (it would fill the run table otherwise)
 };
+// The ingested-behind tier (allow-ingest-behind shards) stays below everything else: only COMPACT_LEVEL and
+// COMPACT_BEHIND take its runs as inputs, the other modes plan over the newer runs alone.  On such shards no output is
+// bottom-most (RocksDB: bottommost_level_ = bottommost_level() && !allow_ingest_behind): tombstones are kept, and merge
+// operands without a base below them stay operands, because a later ingest may put data under them.
 
 // Which runs are merged?  Size-tiered (the role of RocksDB's level0_file_num_compaction_trigger + level sizing,
 // examples/counter_service/rocksdb_options.cpp:82-93): at the trigger the newest runs are merged, stopping before a
@@ -455,17 +481,51 @@ static size_t unpinned_runs(const rsp_shard* s) {
 
 static void bg_request(rsp_engine* e, rsp_shard* s);
 
+// the work buffers of a job whose sources are set (n_src, src_n, seg_start, n_items, items_len, n_tiles)
+// (out of device memory: the buffers taken so far go back to the arena before the exception leaves)
+static void alloc_job_work(Arena& a, CompactJob* j, JobHost* h) {
+  const u32 ns = j->n_src;
+  h->items_b = (size_t)std::max<u32>(1, j->items_len) * sizeof(SortItem);
+  h->items2_b = ns > 1 ? (size_t)std::max<u32>(1, j->n_items) * sizeof(SortItem) : 0;
+  h->coranks_b = ns > 1 ? (size_t)(j->n_tiles + 1) * ns * 4 : 0;
+  h->keep_b = (size_t)std::max<u32>(1, j->n_items) * 4;
+  h->fold_b = (size_t)std::max<u32>(1, j->n_items) * 8;
+  j->items = nullptr; j->items2 = nullptr; j->coranks = nullptr;
+  j->keep_units = nullptr; j->out_pos = nullptr; j->out_ord = nullptr; j->fold_val = nullptr;
+  try {
+    j->items = (SortItem*)a.alloc(h->items_b);
+    j->items2 = ns > 1 ? (SortItem*)a.alloc(h->items2_b) : nullptr;
+    j->coranks = ns > 1 ? (u32*)a.alloc(h->coranks_b) : nullptr;
+    j->keep_units = (u32*)a.alloc(h->keep_b);
+    j->out_pos = (u32*)a.alloc(h->keep_b);
+    j->out_ord = (u32*)a.alloc(h->keep_b);
+    j->fold_val = (u64*)a.alloc(h->fold_b);
+  } catch (...) {
+    if (j->items) a.release(j->items, h->items_b);
+    if (j->items2) a.release(j->items2, h->items2_b);
+    if (j->coranks) a.release(j->coranks, h->coranks_b);
+    if (j->keep_units) a.release(j->keep_units, h->keep_b);
+    if (j->out_pos) a.release(j->out_pos, h->keep_b);
+    if (j->out_ord) a.release(j->out_ord, h->keep_b);
+    throw;
+  }
+  j->sorted = ns > 1 ? j->items2 : j->items;
+}
+
 // ---- plan (engine mutex held) ------------------------------------------------------------------------
 static void plan_jobs(rsp_engine* e, const std::vector<rsp_shard*>& shards, CompactMode mode, CompactPlan* plan) {
   Arena& a = e->arena;
   for (rsp_shard* s : shards) {
-    const bool has_mem = mode != COMPACT_MERGE && s->h.mt_count > 0;
-    size_t n_merged = 0;
-    const size_t avail = unpinned_runs(s);
-    if (mode == COMPACT_FULL) n_merged = s->runs.size();  // (the caller waited for the shard's background merge)
+    const bool has_mem = mode != COMPACT_MERGE && mode != COMPACT_BEHIND && s->h.mt_count > 0;
+    size_t n_merged = 0, first = 0;
+    const size_t n_behind = behind_runs(s), n_reg = s->runs.size() - n_behind;
+    const size_t avail = std::min(unpinned_runs(s), n_reg);
+    if (mode == COMPACT_FULL) n_merged = n_reg;  // (the caller waited for the shard's background merge)
+    else if (mode == COMPACT_LEVEL) n_merged = s->runs.size();
+    else if (mode == COMPACT_BEHIND) { first = n_reg; n_merged = n_behind; }
     else if (mode == COMPACT_MERGE) {
-      if (s->merging || s->runs.size() < e->cfg.l0_compaction_trigger) continue;
-      n_merged = tiered_set(s, 0, s->runs.size(), false);
+      if (s->merging || n_reg < e->cfg.l0_compaction_trigger) continue;
+      n_merged = tiered_set(s, 0, n_reg, false);
       if (n_merged < 2) continue;
     } else if (mode == COMPACT_FLUSH && s->runs.size() + 1 > RSP_MAX_RUNS - 1) {
       // merges belong to the background thread; the foreground only merges when the run table itself fills up
@@ -473,11 +533,12 @@ static void plan_jobs(rsp_engine* e, const std::vector<rsp_shard*>& shards, Comp
     }
     // the run table must never overflow: if the flush would, everything is merged right here (a background merge of
     // some of these runs then finds its sources gone at install time and drops its output)
-    if (mode == COMPACT_FLUSH && has_mem && s->runs.size() - n_merged + 1 > RSP_MAX_RUNS) n_merged = s->runs.size();
-    const bool full = n_merged == s->runs.size();
+    if (mode == COMPACT_FLUSH && has_mem && s->runs.size() - n_merged + 1 > RSP_MAX_RUNS) n_merged = n_reg;
+    const bool full = first == 0 && n_merged == s->runs.size();
     if (!has_mem && n_merged <= 1) {
-      // nothing to flush; a single run is already fully compacted unless it holds tombstones
-      if (!(mode == COMPACT_FULL && s->runs.size() == 1)) continue;
+      // nothing to flush; a single run is already fully compacted unless it holds tombstones (or, for change_level,
+      // is a behind run)
+      if (!((mode == COMPACT_FULL || mode == COMPACT_LEVEL) && n_merged == 1)) continue;
     }
     CompactJob j;
     memset(&j, 0, sizeof(j));
@@ -488,7 +549,7 @@ static void plan_jobs(rsp_engine* e, const std::vector<rsp_shard*>& shards, Comp
       j.src_is_mem[ns] = 1; ns++;
       j.n_pow2 = next_pow2(std::max<u32>(2, s->h.mt_count));
     }
-    for (size_t r = 0; r < n_merged; r++) {
+    for (size_t r = first; r < first + n_merged; r++) {
       auto& run = s->runs[r];
       j.src_heap[ns] = run->heap; j.src_ent_off[ns] = run->ent_off; j.src_n[ns] = run->n_ent; j.src_is_mem[ns] = 0;
       ns++;
@@ -504,22 +565,10 @@ static void plan_jobs(rsp_engine* e, const std::vector<rsp_shard*>& shards, Comp
     j.n_items = (u32)n;
     j.items_len = (u32)at;
     j.n_tiles = ns > 1 ? (u32)((n + MERGE_TILE - 1) / MERGE_TILE) : 0;
-    j.bottom = (full && mode != COMPACT_SNAPSHOT) ? 1 : 0;
+    j.bottom = (full && mode != COMPACT_SNAPSHOT && !(s->open_flags & RSP_SHARD_ALLOW_INGEST_BEHIND)) ? 1 : 0;
     j.merge_op = s->opts.merge_op;
     j.merge_delim = s->h.merge_delim;
-    h.items_b = (size_t)std::max<u32>(1, j.items_len) * sizeof(SortItem);
-    h.items2_b = ns > 1 ? (size_t)std::max<u32>(1, j.n_items) * sizeof(SortItem) : 0;
-    h.coranks_b = ns > 1 ? (size_t)(j.n_tiles + 1) * ns * 4 : 0;
-    h.keep_b = (size_t)std::max<u32>(1, j.n_items) * 4;
-    h.fold_b = (size_t)std::max<u32>(1, j.n_items) * 8;
-    j.items = (SortItem*)a.alloc(h.items_b);
-    j.items2 = ns > 1 ? (SortItem*)a.alloc(h.items2_b) : nullptr;
-    j.coranks = ns > 1 ? (u32*)a.alloc(h.coranks_b) : nullptr;
-    j.sorted = ns > 1 ? j.items2 : j.items;
-    j.keep_units = (u32*)a.alloc(h.keep_b);
-    j.out_pos = (u32*)a.alloc(h.keep_b);
-    j.out_ord = (u32*)a.alloc(h.keep_b);
-    j.fold_val = (u64*)a.alloc(h.fold_b);
+    alloc_job_work(a, &j, &h);
     if (mode == COMPACT_MERGE) {
       s->merging = true;
       s->bg_first_pinned = h.srcs.front().get();
@@ -642,6 +691,11 @@ static void install_jobs(rsp_engine* e, CompactPlan* plan, CompactMode mode) {
       s->stats.compactions++;
       s->runs.erase(s->runs.begin() + at, s->runs.begin() + at + h.n_merged);
     }
+    plan->outs[i]->behind = mode == COMPACT_BEHIND;
+    for (auto& r : h.srcs) {
+      plan->outs[i]->seq0 |= r->seq0 || r->behind;
+      if (mode == COMPACT_BEHIND) plan->outs[i]->file_ranges.insert(plan->outs[i]->file_ranges.end(), r->file_ranges.begin(), r->file_ranges.end());
+    }
     if (plan->outs[i]->n_ent) s->runs.insert(s->runs.begin() + at, plan->outs[i]);
     if (h.has_mem) {
       s->h.mt_tail = 0;
@@ -656,15 +710,20 @@ static void install_jobs(rsp_engine* e, CompactPlan* plan, CompactMode mode) {
   e->last_ms["compact_total"] += plan->ms;  // kernels of every flush / merge so far (sizing round trip included)
   for (u32 i = 0; i < nj; i++) {
     rsp_shard* s = plan->jh[i].s;
-    if (s && s->runs.size() >= e->cfg.l0_compaction_trigger && !s->merging) bg_request(e, s);
+    if (s && s->runs.size() - behind_runs(s) >= e->cfg.l0_compaction_trigger && !s->merging) bg_request(e, s);
   }
 }
 
-// foreground flush / full compaction of a set of shards in one batched pass (engine mutex held throughout)
-static void compact_shards(rsp_engine* e, const std::vector<rsp_shard*>& shards, bool force_full) {
+// foreground flush / compaction (COMPACT_FLUSH, _FULL, _LEVEL or _BEHIND) of a set of shards in one batched pass
+// (engine mutex held throughout)
+static void compact_shards(rsp_engine* e, const std::vector<rsp_shard*>& shards, CompactMode mode) {
   CompactPlan plan;
-  const CompactMode mode = force_full ? COMPACT_FULL : COMPACT_FLUSH;
-  plan_jobs(e, shards, mode, &plan);
+  try {
+    plan_jobs(e, shards, mode, &plan);
+  } catch (...) {  // the work buffers of the jobs planned so far go back
+    release_work(e, &plan);
+    throw;
+  }
   if (plan.jobs.empty()) return;
   wait_readers(e);
   try {
@@ -718,7 +777,7 @@ static void pin_view(rsp_engine* e, rsp_shard* s, std::vector<std::shared_ptr<Ru
   pinned->insert(pinned->end(), s->runs.begin(), s->runs.end());
   if (pinned->size() > RSP_MAX_RUNS) {  // the view has room for RSP_MAX_RUNS runs: fold the memtable in after all
     pinned->clear();
-    compact_shards(e, {s}, false);
+    compact_shards(e, {s}, COMPACT_FLUSH);
     *pinned = s->runs;
   }
   view_of(s, *pinned, v);
@@ -1065,7 +1124,7 @@ static int reserve_for(rsp_engine* e, const rsp_staged* sg) {
     if (s->inflight_units || s->inflight_ents) return -1;  // the mirror lags the device: neither flush nor re-size now
     if (s->h.mt_count) to_flush.push_back(s);
   }
-  if (!to_flush.empty()) { compact_shards(e, to_flush, false); did_work = true; }
+  if (!to_flush.empty()) { compact_shards(e, to_flush, COMPACT_FLUSH); did_work = true; }
   UploadBatch up;
   try {
     for (size_t g = 0; g < sg->group_shard.size(); g++) {
@@ -2151,7 +2210,7 @@ void rsp_engine_destroy(rsp_engine* e) {
   for (rsp_shard* s : e->slots)
     if (s) { s->runs.clear(); delete s; }
   e->arena.destroy();
-  e->pin_in.destroy(); e->pin_out.destroy(); e->pin_up.destroy(); e->pin_totals.destroy(); e->dev_up.destroy(); e->dev_tick.destroy(); e->dev_q.destroy(); e->dev_pending.destroy();
+  e->pin_in.destroy(); e->pin_out.destroy(); e->pin_up.destroy(); e->pin_totals.destroy(); e->pin_ingest.destroy(); e->dev_up.destroy(); e->dev_tick.destroy(); e->dev_q.destroy(); e->dev_pending.destroy();
   cudaFree(e->d_shards);
   cudaFree(e->d_fast);
   cudaEventDestroy(e->ev0); cudaEventDestroy(e->ev1); cudaEventDestroy(e->up_ev); cudaEventDestroy(e->pending_ev);
@@ -2165,8 +2224,8 @@ void rsp_engine_destroy(rsp_engine* e) {
 int rsp_engine_device(const rsp_engine* e) { return e->device; }
 void* rsp_engine_stream(const rsp_engine* e) { return (void*)e->st; }
 
-static int shard_open_locked(rsp_engine* e, const char* name, const rsp_shard_opts* opts, rsp_shard** out) {
-  if (e->by_name.count(name)) return RSP_INVALID_ARGUMENT;
+static int shard_open_locked(rsp_engine* e, const char* name, const rsp_shard_opts* opts, uint32_t flags, rsp_shard** out) {
+  if (e->by_name.count(name) || (flags & ~(uint32_t)RSP_SHARD_ALLOW_INGEST_BEHIND)) return RSP_INVALID_ARGUMENT;
   if (opts && opts->merge_op == RSP_MERGE_STRING_APPEND && (opts->merge_delim & ~0x1ffu)) return RSP_INVALID_ARGUMENT;
   u32 ix = 0;
   while (ix < e->slots.size() && e->slots[ix]) ix++;
@@ -2176,6 +2235,7 @@ static int shard_open_locked(rsp_engine* e, const char* name, const rsp_shard_op
   static std::atomic<u64> next_uid{1};
   s->uid = next_uid++;
   s->eng = e; s->name = name; s->index = ix;
+  s->open_flags = flags;
   memset(&s->opts, 0, sizeof(s->opts));
   if (opts) s->opts = *opts;
   memset(&s->h, 0, sizeof(s->h));
@@ -2215,13 +2275,16 @@ static void shard_close_locked(rsp_shard* s) {
   delete s;
 }
 
-int rsp_shard_open(rsp_engine* e, const char* name, const rsp_shard_opts* opts, rsp_shard** out) {
+int rsp_shard_open_ex(rsp_engine* e, const char* name, const rsp_shard_opts* opts, uint32_t flags, rsp_shard** out) {
   try {
   if (!e || !name || !out) return RSP_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(e->mu);
   CUDA_OK(cudaSetDevice(e->device));
-  return shard_open_locked(e, name, opts, out);
+  return shard_open_locked(e, name, opts, flags, out);
   } catch (...) { return abi_caught(); }
+}
+int rsp_shard_open(rsp_engine* e, const char* name, const rsp_shard_opts* opts, rsp_shard** out) {
+  return rsp_shard_open_ex(e, name, opts, 0, out);
 }
 
 int rsp_shard_close(rsp_shard* s) {
@@ -2252,12 +2315,128 @@ static void run_key_range(rsp_engine* e, const Run& r, std::string* first, std::
   (void)e;
 }
 
+// host bytes -> device through the engine's pinned staging buffer, in bounded chunks: two halves, so that copying the
+// next chunk into one half overlaps the transfer of the other
+static void upload_staged(rsp_engine* e, void* dst, const void* src, size_t bytes, cudaEvent_t half_done[2]) {
+  const size_t CH = 8u << 20;
+  u8* pin = (u8*)e->pin_ingest.get(2 * CH);
+  for (size_t at = 0, k = 0; at < bytes; at += CH, k ^= 1) {
+    const size_t len = std::min(CH, bytes - at);
+    CUDA_OK(cudaEventSynchronize(half_done[k]));
+    memcpy(pin + k * CH, (const u8*)src + at, len);
+    CUDA_OK(cudaMemcpyAsync((u8*)dst + at, pin + k * CH, len, cudaMemcpyHostToDevice, e->st));
+    CUDA_OK(cudaEventRecord(half_done[k], e->st));
+  }
+}
+
+// n sorted Puts -> one run at sequence 0.  The keys, values and offsets are uploaded once; k_ingest_* write them in the
+// run entry layout into a source heap, which the compaction passes (one pre-sorted source: no sort, no merge) turn into
+// the run with its restart array, block index and hash index.  Nothing reads sequence numbers inside a run against
+// anything but a snapshot bound, which sequence 0 always meets: recency between runs is the run order.  `units`: the
+// source heap's size (n + the key and value units).  On failure the work buffers go back to the arena.
+static std::shared_ptr<Run> build_sorted_run(rsp_engine* e, rsp_shard* s, size_t n, const uint8_t* keys,
+                                             const uint64_t* koff, const uint8_t* vals, const uint64_t* voff, u64 units) {
+  Arena& a = e->arena;
+  const size_t kb = std::max<size_t>(1, koff[n] - koff[0]), vb = std::max<size_t>(1, voff[n] - voff[0]);
+  const size_t ob = (n + 1) * 8, eb = n * 4, tb = (size_t)ingest_tiles((u32)n) * 4, hb = units * 16;
+  IngestArgs g{};
+  CompactPlan plan;
+  cudaEvent_t half_done[2] = {nullptr, nullptr};
+  auto release_inputs = [&] {
+    for (cudaEvent_t ev : half_done) if (ev) cudaEventDestroy(ev);
+    if (g.keys) a.release((void*)g.keys, kb);
+    if (g.vals) a.release((void*)g.vals, vb);
+    if (g.koff) a.release((void*)g.koff, ob);
+    if (g.voff) a.release((void*)g.voff, ob);
+    if (g.ent_off) a.release(g.ent_off, eb);
+    if (g.tile_sum) a.release(g.tile_sum, tb);
+    if (g.heap) a.release(g.heap, hb);
+  };
+  try {
+    for (cudaEvent_t& ev : half_done) {
+      CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+      CUDA_OK(cudaEventRecord(ev, e->st));
+    }
+    g.n = (u32)n;
+    g.keys = (const u8*)a.alloc(kb);
+    g.vals = (const u8*)a.alloc(vb);
+    g.koff = (const u64*)a.alloc(ob);
+    g.voff = (const u64*)a.alloc(ob);
+    g.ent_off = (u32*)a.alloc(eb);
+    g.tile_sum = (u32*)a.alloc(tb);
+    g.heap = (u8*)a.alloc(hb);
+    upload_staged(e, (void*)g.keys, keys + koff[0], koff[n] - koff[0], half_done);
+    upload_staged(e, (void*)g.vals, vals + voff[0], voff[n] - voff[0], half_done);
+    upload_staged(e, (void*)g.koff, koff, ob, half_done);
+    upload_staged(e, (void*)g.voff, voff, ob, half_done);
+    launch_ingest_entries(g, e->st);
+    CUDA_OK(cudaGetLastError());
+    e->launches += 3;
+    CompactJob j;
+    memset(&j, 0, sizeof(j));
+    j.src_heap[0] = g.heap; j.src_ent_off[0] = g.ent_off; j.src_n[0] = (u32)n; j.src_is_mem[0] = 0;
+    j.n_src = 1; j.n_items = (u32)n; j.items_len = (u32)n;
+    j.merge_op = s->opts.merge_op;
+    j.merge_delim = s->h.merge_delim;
+    JobHost h{s, s->index, s->uid, true, false, 0, {}, 0, 0, 0, 0, 0};
+    alloc_job_work(a, &j, &h);
+    plan.jh.push_back(h);
+    plan.jobs.push_back(j);
+    run_jobs(e, &plan, e->st, e->ev0, e->ev1, &e->pin_totals);
+  } catch (...) {
+    cudaStreamSynchronize(e->st);
+    release_work(e, &plan);
+    release_inputs();
+    throw;
+  }
+  release_work(e, &plan);
+  release_inputs();
+  e->last_ms["ingest"] = plan.ms;
+  return plan.outs[0];
+}
+
+// The checks both ingest forms share, before anything changes: keys strictly increasing, every entry within the
+// compaction's 24-bit entry size and the source heap within the run format's 32-bit unit offsets.  *units: the heap's
+// size.
+static int check_sorted_input(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_t* koff, const uint64_t* voff,
+                              u64* units) {
+  u64 u = 0;
+  for (size_t i = 0; i < n; i++) {
+    const size_t bl = (size_t)(koff[i + 1] - koff[i]);
+    const u64 eu = 1 + ((u64)bl + 15) / 16 + ((u64)(voff[i + 1] - voff[i]) + 15) / 16;
+    if (eu > 0xffffffu) { set_err(s, "Invalid argument: entry too large"); return RSP_INVALID_ARGUMENT; }
+    u += eu;
+    if (i == 0) continue;
+    const size_t al = (size_t)(koff[i] - koff[i - 1]);
+    const int c = memcmp(keys + koff[i - 1], keys + koff[i], std::min(al, bl));
+    if (c > 0 || (c == 0 && al >= bl)) { set_err(s, "Invalid argument: Keys must be added in order"); return RSP_INVALID_ARGUMENT; }
+  }
+  if (n > 0xffffffffull || u > 0xffffffffull) { set_err(s, "Invalid argument: file too large for one run"); return RSP_INVALID_ARGUMENT; }
+  *units = u;
+  return RSP_OK;
+}
+
+// publish a changed run list of the shard (engine mutex held)
+static void publish_runs(rsp_engine* e, rsp_shard* s) {
+  UploadBatch up;
+  stage_upload(e, s, false, false, &up);
+  commit_uploads(e, &up);
+  note_mutation(e);
+  CUDA_OK(cudaStreamSynchronize(e->st));
+}
+
+static bool ranges_overlap(rsp_engine* e, const Run& r, const std::string& lo, const std::string& hi) {
+  if (!r.n_ent) return false;
+  std::string rf, rl;
+  run_key_range(e, r, &rf, &rl);
+  return !(hi < rf) && !(rl < lo);
+}
+
 // DB::IngestExternalFile for a sorted set of Puts (rocksdb_admin/admin_handler.cpp:1820-1845, sequence rules of
 // rocksdb_replicator/tests/rocksdb_assumption_test.cpp:248-283): the keys become ONE new sorted run.  When its key
 // range intersects existing data the run is newer than everything and the shard's sequence number advances by one
-// (refused unless allow_global_seqno); otherwise the sequence number does not move.  The run is produced by the
-// ordinary apply + flush kernels on a scratch shard and then handed to the target (sequence numbers inside runs are
-// not consulted by reads: recency is the run order).
+// (refused unless allow_global_seqno); otherwise the sequence number does not move and the run holds sequence-0 data.
+// The run is built on the device from the sorted input (build_sorted_run).
 int rsp_ingest_sorted(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_t* koff, const uint8_t* vals,
                       const uint64_t* voff, int allow_global_seqno, uint64_t* seq_out) {
   try {
@@ -2265,25 +2444,17 @@ int rsp_ingest_sorted(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_
   rsp_engine* e = s->eng;
   std::lock_guard<std::mutex> g(e->mu);
   CUDA_OK(cudaSetDevice(e->device));
-  auto key = [&](size_t i) { return std::string((const char*)keys + koff[i], (size_t)(koff[i + 1] - koff[i])); };
-  for (size_t i = 1; i < n; i++) {
-    const size_t al = (size_t)(koff[i] - koff[i - 1]), bl = (size_t)(koff[i + 1] - koff[i]);
-    const int c = memcmp(keys + koff[i - 1], keys + koff[i], std::min(al, bl));
-    if (c > 0 || (c == 0 && al >= bl)) { set_err(s, "Invalid argument: Keys must be added in order"); return RSP_INVALID_ARGUMENT; }
-  }
+  u64 units = 0;
+  if (int rc = check_sorted_input(s, n, keys, koff, voff, &units)) return rc;
   if (s->latch) return (int)(s->latch >> 8);
   if (ticks_in_flight(s)) return RSP_BUSY;
   // everything the shard holds must be in runs before ranges are compared
-  if (s->h.mt_count) compact_shards(e, {s}, false);
-  if (s->runs.size() + 1 > RSP_MAX_RUNS) compact_shards(e, {s}, true);
-  const std::string lo = key(0), hi = key(n - 1);
+  if (s->h.mt_count) compact_shards(e, {s}, COMPACT_FLUSH);
+  if (s->runs.size() + 1 > RSP_MAX_RUNS) compact_shards(e, {s}, COMPACT_FULL);
+  const std::string lo((const char*)keys + koff[0], (size_t)(koff[1] - koff[0]));
+  const std::string hi((const char*)keys + koff[n - 1], (size_t)(koff[n] - koff[n - 1]));
   bool overlap = false;
-  for (auto& r : s->runs) {
-    if (!r->n_ent) continue;
-    std::string rf, rl;
-    run_key_range(e, *r, &rf, &rl);
-    if (!(hi < rf) && !(rl < lo)) { overlap = true; break; }
-  }
+  for (auto& r : s->runs) if ((overlap = ranges_overlap(e, *r, lo, hi))) break;
   // IngestExternalFileOptions::snapshot_consistency (default true): with a snapshot live the file takes a global
   // sequence number even when it overlaps nothing, so that it is newer than every snapshot
   const bool global_seqno = overlap || s->n_snapshots > 0;
@@ -2291,63 +2462,80 @@ int rsp_ingest_sorted(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_
     set_err(s, "Invalid argument: Global seqno is required, but disabled");
     return RSP_INVALID_ARGUMENT;
   }
-  // build the run on a scratch shard with the ordinary apply + flush path
-  rsp_shard* tmp = nullptr;
-  rsp_shard_opts so;
-  memset(&so, 0, sizeof(so));
-  size_t payload = (size_t)koff[n] + (size_t)voff[n];
-  so.write_buffer_bytes = payload + n * 64 + (1u << 20);
-  static std::atomic<u64> ctr{0};
-  const std::string tname = "__ingest_" + std::to_string(ctr++);
-  int rc = shard_open_locked(e, tname.c_str(), &so, &tmp);
-  if (rc != RSP_OK) return rc;
-  const size_t CH = 1u << 16;
-  for (size_t c0 = 0; c0 < n && rc == RSP_OK; c0 += CH) {
-    const size_t cn = std::min(CH, n - c0);
-    std::string blob;
-    std::vector<uint64_t> off(cn + 1, 0);
-    std::vector<uint32_t> six(cn, tmp->index);
-    for (size_t i = 0; i < cn; i++) {
-      const std::string k = key(c0 + i);
-      const size_t vl = (size_t)(voff[c0 + i + 1] - voff[c0 + i]);
-      off[i] = blob.size();
-      blob.append(8, '\0');
-      const uint32_t one = 1;
-      blob.append((const char*)&one, 4);
-      blob.push_back(0x1);
-      for (uint32_t v = (uint32_t)k.size(); ; v >>= 7) { if (v >= 128) blob.push_back((char)((v & 127) | 128)); else { blob.push_back((char)v); break; } }
-      blob.append(k);
-      for (uint32_t v = (uint32_t)vl; ; v >>= 7) { if (v >= 128) blob.push_back((char)((v & 127) | 128)); else { blob.push_back((char)v); break; } }
-      blob.append((const char*)vals + voff[c0 + i], vl);
-    }
-    off[cn] = blob.size();
-    blob.push_back('\0');
-    std::vector<int32_t> st(cn, 0);
-    rc = apply_many_locked(e, cn, six.data(), (const uint8_t*)blob.data(), off.data(), nullptr, st.data());
+  wait_readers(e);
+  std::shared_ptr<Run> run = build_sorted_run(e, s, n, keys, koff, vals, voff, units);
+  run->seq0 = !global_seqno;
+  if (run->n_ent) s->runs.insert(s->runs.begin(), run);
+  if (global_seqno) {
+    const u64 seq = s->last_seq.load() + 1;
+    s->h.last_seq = seq;
+    s->h.pub_seq = seq;
+    s->last_seq.store(seq, std::memory_order_release);
   }
-  if (rc == RSP_OK) {
-    compact_shards(e, {tmp}, false);
-    if (tmp->runs.size() > 1) compact_shards(e, {tmp}, true);
-    if (!tmp->runs.empty()) {
-      s->runs.insert(s->runs.begin(), tmp->runs[0]);
-      tmp->runs.clear();
-    }
-    if (global_seqno) {
-      const u64 seq = s->last_seq.load() + 1;
-      s->h.last_seq = seq;
-      s->h.pub_seq = seq;
-      s->last_seq.store(seq, std::memory_order_release);
-    }
-    UploadBatch up;
-    stage_upload(e, s, false, false, &up);
-    commit_uploads(e, &up);
-    note_mutation(e);
-    CUDA_OK(cudaStreamSynchronize(e->st));
-  }
-  shard_close_locked(tmp);
+  publish_runs(e, s);
   if (seq_out) *seq_out = s->last_seq.load();
-  return rc;
+  return RSP_OK;
   } catch (...) { return abi_caught(); }
+}
+
+// IngestExternalFileOptions::ingest_behind (RocksDB 5.7): the keys become a run of the shard's ingested-behind tier,
+// below everything the shard holds; see include/rsp_b200.h for the rules and refusals.
+int rsp_ingest_sorted_behind(rsp_shard* s, size_t n, const uint8_t* keys, const uint64_t* koff, const uint8_t* vals,
+                             const uint64_t* voff) {
+  try {
+  if (!s || !n || !keys || !koff || !voff) return RSP_INVALID_ARGUMENT;
+  rsp_engine* e = s->eng;
+  std::lock_guard<std::mutex> g(e->mu);
+  CUDA_OK(cudaSetDevice(e->device));
+  u64 units = 0;
+  if (int rc = check_sorted_input(s, n, keys, koff, voff, &units)) return rc;
+  if (!(s->open_flags & RSP_SHARD_ALLOW_INGEST_BEHIND)) {
+    set_err(s, "Invalid argument: can't ingest_behind file in DB with allow_ingest_behind=false");
+    return RSP_INVALID_ARGUMENT;
+  }
+  if (s->latch) return (int)(s->latch >> 8);
+  if (ticks_in_flight(s)) return RSP_BUSY;
+  if (s->n_snapshots) {  // RocksDB would show the file to the live snapshots; a pinned view cannot grow a run
+    set_err(s, "Not implemented: ingest_behind while the shard has live snapshots");
+    return RSP_NOT_SUPPORTED;
+  }
+  const size_t n_behind = behind_runs(s), n_reg = s->runs.size() - n_behind;
+  const std::string lo((const char*)keys + koff[0], (size_t)(koff[1] - koff[0]));
+  const std::string hi((const char*)keys + koff[n - 1], (size_t)(koff[n] - koff[n - 1]));
+  for (size_t i = n_reg; i < s->runs.size(); i++)
+    for (const auto& f : s->runs[i]->file_ranges)
+      if (!(hi < f.first) && !(f.second < lo)) {
+        set_err(s, "Invalid argument: Can't ingest_behind file as it doesn't fit at the bottommost level!");
+        return RSP_INVALID_ARGUMENT;
+      }
+  for (size_t i = 0; i < n_reg; i++)
+    if (s->runs[i]->seq0) {
+      set_err(s, "Invalid argument: Can't ingest_behind file as despite allow_ingest_behind=true there are files with 0 "
+                 "seqno in database at upper levels!");
+      return RSP_INVALID_ARGUMENT;
+    }
+  // room in the run table: the tier holds at most BEHIND_MAX_RUNS runs (they are merged with each other before a file
+  // would make one more), so the newer runs keep RSP_MAX_RUNS - BEHIND_MAX_RUNS slots of the table
+  if (s->runs.size() + 1 > RSP_MAX_RUNS) compact_shards(e, {s}, COMPACT_FULL);
+  if (behind_runs(s) + 1 > BEHIND_MAX_RUNS) compact_shards(e, {s}, COMPACT_BEHIND);
+  wait_readers(e);
+  std::shared_ptr<Run> run = build_sorted_run(e, s, n, keys, koff, vals, voff, units);
+  run->behind = run->seq0 = true;
+  run->file_ranges.emplace_back(lo, hi);
+  if (run->n_ent) s->runs.push_back(run);
+  publish_runs(e, s);
+  return RSP_OK;
+  } catch (...) { return abi_caught(); }
+}
+
+uint64_t rsp_shard_behind_bytes(const rsp_shard* s) {
+  try {
+  if (!s) return 0;
+  std::lock_guard<std::mutex> g(s->eng->mu);
+  u64 b = 0;
+  for (size_t i = s->runs.size() - behind_runs(s); i < s->runs.size(); i++) b += s->runs[i]->bytes();
+  return b;
+  } catch (...) { abi_caught(); return 0; }
 }
 
 uint32_t rsp_shard_index(const rsp_shard* s) { return s->index; }
@@ -2705,21 +2893,22 @@ int rsp_flush(rsp_shard* s) {
   std::lock_guard<std::mutex> g(e->mu);
   if (ticks_in_flight(s)) return RSP_BUSY;
   CUDA_OK(cudaSetDevice(e->device));
-  compact_shards(e, {s}, false);
+  compact_shards(e, {s}, COMPACT_FLUSH);
   return RSP_OK;
   } catch (...) { return abi_caught(); }
 }
-int rsp_compact(rsp_shard* s) {
+int rsp_compact_ex(rsp_shard* s, uint32_t flags) {
   try {
-  if (!s) return RSP_INVALID_ARGUMENT;
+  if (!s || (flags & ~(uint32_t)RSP_COMPACT_CHANGE_LEVEL)) return RSP_INVALID_ARGUMENT;
   rsp_engine* e = s->eng;
   std::lock_guard<std::mutex> g(e->mu);
   if (ticks_in_flight(s)) return RSP_BUSY;
   CUDA_OK(cudaSetDevice(e->device));
-  compact_shards(e, {s}, true);
+  compact_shards(e, {s}, (flags & RSP_COMPACT_CHANGE_LEVEL) ? COMPACT_LEVEL : COMPACT_FULL);
   return RSP_OK;
   } catch (...) { return abi_caught(); }
 }
+int rsp_compact(rsp_shard* s) { return rsp_compact_ex(s, 0); }
 static int all_shards(rsp_engine* e, bool full) {
   std::lock_guard<std::mutex> g(e->mu);
   CUDA_OK(cudaSetDevice(e->device));
@@ -2731,7 +2920,7 @@ static int all_shards(rsp_engine* e, bool full) {
   std::vector<rsp_shard*> part;
   u64 part_bytes = 0;
   auto run_part = [&] {
-    if (!part.empty()) compact_shards(e, part, full);
+    if (!part.empty()) compact_shards(e, part, full ? COMPACT_FULL : COMPACT_FLUSH);
     part.clear();
     part_bytes = 0;
   };
@@ -3073,7 +3262,7 @@ static int multi_scan_host(rsp_engine* e, size_t n, const uint32_t* shard_ix, rs
       if (ticks_in_flight(s)) return RSP_BUSY;
       if (s->h.mt_count && std::find(fl.begin(), fl.end(), s) == fl.end()) fl.push_back(s);
     }
-    if (!fl.empty()) compact_shards(e, fl, false);
+    if (!fl.empty()) compact_shards(e, fl, COMPACT_FLUSH);
   }
   std::vector<uint64_t> no_keys;
   if (from_extreme) { no_keys.assign(n + 1, 0); koff = no_keys.data(); }

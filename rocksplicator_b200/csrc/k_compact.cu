@@ -19,6 +19,8 @@
 //   k_compact_write : copy / synthesise the kept entries into the new heap, write the restart array
 //                     (ent_off), the block index (first-key prefix per 32 entries) and the bucketised
 //                     hash index
+//   k_ingest_*      : an ingested file (sorted Puts) written straight into a source heap in the run entry layout; the
+//                     passes above then build its run from that one pre-sorted source (no sort, no merge)
 #include <algorithm>
 #include <atomic>
 
@@ -610,6 +612,118 @@ __global__ void __launch_bounds__(256) k_compact_write(const CompactJob* jobs) {
       bucket = bucket + 1 == j.out_n_buckets ? 0 : bucket + 1;
     }
   }
+}
+
+// ---- ingestion: sorted Puts -> a source heap in the run entry layout ------------------------------------------
+// k_ingest_size   : one CTA per INGEST_TILE entries, eight consecutive entries per thread: each entry's size in units,
+//                   scanned within the tile (ent_off holds the offset inside the tile, tile_sum the tile's total)
+// k_ingest_scan   : one CTA: exclusive scan of the tile totals
+// k_ingest_write  : eight lanes per entry, one 16-byte unit per lane and step: the header (sequence 0, kTypeValue),
+//                   then the key and the value, each zero padded to whole units; ent_off becomes the heap offset
+constexpr u32 IG_THREADS = 256;
+constexpr u32 IG_PER = INGEST_TILE / IG_THREADS;
+constexpr u32 IG_LANES = 8;
+
+__global__ void __launch_bounds__(IG_THREADS) k_ingest_size(IngestArgs a) {
+  __shared__ u32 s_warp[IG_THREADS / 32];
+  const u32 tid = threadIdx.x, lane = tid & 31u, wid = tid >> 5;
+  const u32 i0 = blockIdx.x * INGEST_TILE + tid * IG_PER;
+  u32 u[IG_PER], sum = 0;
+#pragma unroll
+  for (u32 k = 0; k < IG_PER; k++) {
+    const u32 i = i0 + k;
+    u[k] = i < a.n ? 1u + units_of((u32)(a.koff[i + 1] - a.koff[i])) + units_of((u32)(a.voff[i + 1] - a.voff[i])) : 0u;
+    sum += u[k];
+  }
+  u32 incl = sum;
+#pragma unroll
+  for (u32 d = 1; d < 32; d <<= 1) {
+    const u32 o = __shfl_up_sync(0xffffffffu, incl, d);
+    if (lane >= d) incl += o;
+  }
+  if (lane == 31) s_warp[wid] = incl;
+  __syncthreads();
+  u32 wbase = 0, total = 0;
+#pragma unroll
+  for (u32 w = 0; w < IG_THREADS / 32; w++) {
+    if (w < wid) wbase += s_warp[w];
+    total += s_warp[w];
+  }
+  u32 at = wbase + incl - sum;
+#pragma unroll
+  for (u32 k = 0; k < IG_PER; k++) {
+    if (i0 + k < a.n) a.ent_off[i0 + k] = at;
+    at += u[k];
+  }
+  if (tid == 0) a.tile_sum[blockIdx.x] = total;
+}
+
+__global__ void __launch_bounds__(1024) k_ingest_scan(u32* tile_sum, u32 nt) {
+  __shared__ u32 s_warp[32];
+  __shared__ u32 s_carry;
+  const u32 lane = threadIdx.x & 31u, wid = threadIdx.x >> 5;
+  if (threadIdx.x == 0) s_carry = 0;
+  __syncthreads();
+  for (u32 base = 0; base < nt; base += 1024) {
+    const u32 i = base + threadIdx.x;
+    const u32 v = i < nt ? tile_sum[i] : 0u;
+    u32 incl = v;
+#pragma unroll
+    for (u32 d = 1; d < 32; d <<= 1) {
+      const u32 o = __shfl_up_sync(0xffffffffu, incl, d);
+      if (lane >= d) incl += o;
+    }
+    if (lane == 31) s_warp[wid] = incl;
+    __syncthreads();
+    u32 wbase = 0;
+    for (u32 w = 0; w < wid; w++) wbase += s_warp[w];
+    const u32 carry = s_carry;
+    if (i < nt) tile_sum[i] = carry + wbase + incl - v;
+    __syncthreads();
+    if (threadIdx.x == 1023) s_carry = carry + wbase + incl;
+    __syncthreads();
+  }
+}
+
+__global__ void __launch_bounds__(256) k_ingest_write(IngestArgs a) {
+  const u64 t = (u64)blockIdx.x * blockDim.x + threadIdx.x;
+  const u32 g = (u32)(t / IG_LANES), l = (u32)(t % IG_LANES);  // the entry, this lane within its group
+  const bool valid = g < a.n;
+  const u32 pos = valid ? a.ent_off[g] + a.tile_sum[g / INGEST_TILE] : 0u;
+  __syncwarp();  // every lane of the group has read the tile-local offset before lane 0 replaces it
+  if (!valid) return;
+  if (l == 0) a.ent_off[g] = pos;
+  const u8* key = a.keys + (a.koff[g] - a.koff[0]);
+  const u8* val = a.vals + (a.voff[g] - a.voff[0]);
+  const u32 klen = (u32)(a.koff[g + 1] - a.koff[g]), vlen = (u32)(a.voff[g + 1] - a.voff[g]);
+  const u32 ku = units_of(klen), U = 1u + ku + units_of(vlen);
+  uint4* d = reinterpret_cast<uint4*>(a.heap + (u64)pos * 16u);
+  for (u32 u = l; u < U; u += IG_LANES) {
+    if (u == 0) { d[0] = make_uint4((u32)kTypeValue, 0u, klen, vlen); continue; }  // seqtype = 0 << 8 | kTypeValue
+    const bool in_key = u <= ku;
+    const u8* src = in_key ? key : val;
+    const u32 len = in_key ? klen : vlen;
+    const u32 b0 = (in_key ? u - 1u : u - 1u - ku) * 16u;
+    u32 w[4];
+#pragma unroll
+    for (u32 q = 0; q < 4; q++) {
+      w[q] = 0;
+#pragma unroll
+      for (u32 b = 0; b < 4; b++) {
+        const u32 at = b0 + q * 4u + b;
+        if (at < len) w[q] |= (u32)src[at] << (8u * b);
+      }
+    }
+    d[u] = make_uint4(w[0], w[1], w[2], w[3]);
+  }
+}
+
+void launch_ingest_entries(const IngestArgs& a, cudaStream_t s) {
+  if (!a.n) return;
+  const u32 nt = ingest_tiles(a.n);
+  k_ingest_size<<<nt, IG_THREADS, 0, s>>>(a);
+  k_ingest_scan<<<1, 1024, 0, s>>>(a.tile_sum, nt);
+  k_ingest_write<<<(u32)(((u64)a.n * IG_LANES + 255u) / 256u), 256, 0, s>>>(a);
 }
 
 // ---- maintenance helpers: one launch per batch of shards ---------------------------------------------------

@@ -262,6 +262,25 @@ void launch_compact_write(const CompactJob* d_jobs, u32 n_jobs, u32 max_items, c
 // zero the hash index of every job's output run (out_hslots, out_n_buckets buckets): one launch for the whole batch
 void launch_zero_out_hslots(const CompactJob* d_jobs, u32 n_jobs, u32 max_buckets, cudaStream_t s);
 
+// ---- ingestion: n sorted Puts written straight into a source heap in the run entry layout ----------------------------
+// Entry i is a Put at sequence 0 of key keys[koff[i] - koff[0] ..) and value vals[voff[i] - voff[0] ..): the uploaded
+// bytes, offsets as the caller gave them.  The heap is one pre-sorted, non-memtable compaction source: the compaction
+// passes then build the run's restart array, block index and hash index.
+struct IngestArgs {
+  const u8* keys;
+  const u8* vals;
+  const u64* koff;  // [n+1]
+  const u64* voff;  // [n+1]
+  u32 n;
+  u32* ent_off;     // [n] out: unit offset of entry i (exclusive scan of the entry sizes)
+  u32* tile_sum;    // [ingest_tiles(n)] scratch: units of each INGEST_TILE-entry tile, then their exclusive scan
+  u8* heap;         // the entries (the caller sizes it: n + sum of units_of(klen) + units_of(vlen) units)
+};
+constexpr u32 INGEST_TILE = 2048;
+inline u32 ingest_tiles(u32 n) { return (n + INGEST_TILE - 1) / INGEST_TILE; }
+// three launches: entry sizes scanned per tile, the tile totals scanned, the entries written
+void launch_ingest_entries(const IngestArgs& a, cudaStream_t s);
+
 // ---- batched descriptor upload ------------------------------------------------------------------------
 // One record per shard whose descriptors changed (a flush / merge batch installs up to thousands at once): staged in
 // pinned memory, ONE copy, ONE launch that scatters them — instead of three small pageable copies and a memset per shard.

@@ -15,6 +15,8 @@ SO_PATH = os.path.join(HERE, "librsp_b200.so")
 OK, NOT_FOUND, CORRUPTION, NOT_SUPPORTED, INVALID_ARGUMENT, IO_ERROR = 0, 1, 2, 3, 4, 5
 INCOMPLETE = 7
 MERGE_NONE, MERGE_COUNTER, MERGE_UINT64ADD, MERGE_APPEND, MERGE_CALLBACK, MERGE_STRING_APPEND = 0, 1, 2, 3, 4, 5
+SHARD_ALLOW_INGEST_BEHIND = 1  # rsp_shard_open_ex flags
+COMPACT_CHANGE_LEVEL = 1       # rsp_compact_ex flags
 
 MERGE_FN = C.CFUNCTYPE(C.c_int, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                        C.c_size_t, C.c_void_p, C.c_void_p)
@@ -114,6 +116,10 @@ EXPORTS = {
     "rsp_get_stats": (C.c_int, [C.c_void_p, C.POINTER(Stats)]),
     "rsp_ingest_sorted": (C.c_int, [C.c_void_p, C.c_size_t, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p, C.c_int,
                                     C.POINTER(C.c_uint64)]),
+    "rsp_ingest_sorted_behind": (C.c_int, [C.c_void_p, C.c_size_t, C.c_char_p, C.c_void_p, C.c_char_p, C.c_void_p]),
+    "rsp_shard_behind_bytes": (C.c_uint64, [C.c_void_p]),
+    "rsp_shard_open_ex": (C.c_int, [C.c_void_p, C.c_char_p, C.POINTER(ShardOpts), C.c_uint32, C.POINTER(C.c_void_p)]),
+    "rsp_compact_ex": (C.c_int, [C.c_void_p, C.c_uint32]),
     "rsp_multi_get_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p,
                                        C.c_uint32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "rsp_multi_scan_device": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_uint32, C.c_uint32,
@@ -308,8 +314,10 @@ class Shard:
     """One DB ("segment%05d"): apply == DbWrapper::HandleReplicateResponse, write == WriteToLeader,
     latest_seq == LatestSequenceNumber, get/multi_get/iterator == the ApplicationDB read surface."""
 
-    def __init__(self, engine, name, merge_op=MERGE_NONE, write_buffer_bytes=0, merge_fn=None, merge_delim=None):
-        """merge_delim: MERGE_STRING_APPEND's delimiter, one byte (b"," / b"\\0") or None for plain concatenation"""
+    def __init__(self, engine, name, merge_op=MERGE_NONE, write_buffer_bytes=0, merge_fn=None, merge_delim=None,
+                 allow_ingest_behind=False):
+        """merge_delim: MERGE_STRING_APPEND's delimiter, one byte (b"," / b"\\0") or None for plain concatenation;
+        allow_ingest_behind: DBOptions::allow_ingest_behind (ingest(..., behind=True); no compaction is bottom-most)"""
         self.engine = engine
         self.lib = engine.lib
         self.kind = "b200"
@@ -324,7 +332,8 @@ class Shard:
             self._merge_fn = MERGE_FN(merge_fn)
             opts.merge_fn = C.cast(self._merge_fn, C.c_void_p)
         h = C.c_void_p()
-        rc = self.lib.rsp_shard_open(engine.h, name.encode(), C.byref(opts), C.byref(h))
+        flags = SHARD_ALLOW_INGEST_BEHIND if allow_ingest_behind else 0
+        rc = self.lib.rsp_shard_open_ex(engine.h, name.encode(), C.byref(opts), flags, C.byref(h))
         if rc != OK:
             raise RuntimeError(f"rsp_shard_open({name}) -> {rc}")
         self.h = h
@@ -386,10 +395,17 @@ class Shard:
         return out
 
     def flush(self): return self.lib.rsp_flush(self.h)
-    def compact(self): return self.lib.rsp_compact(self.h)
+    def compact(self, change_level=False):
+        """CompactRange(nullptr, nullptr); change_level=True also folds the ingested-behind tier in"""
+        return self.lib.rsp_compact_ex(self.h, COMPACT_CHANGE_LEVEL if change_level else 0)
 
-    def ingest(self, sorted_kv, allow_global_seqno=True) -> int:
-        """DB::IngestExternalFile for sorted (key, value) pairs (see rocksplicator_b200/sst.py for SST files)"""
+    def behind_bytes(self) -> int:
+        """bytes held by the ingested-behind tier (0: empty)"""
+        return self.lib.rsp_shard_behind_bytes(self.h)
+
+    def ingest(self, sorted_kv, allow_global_seqno=True, behind=False) -> int:
+        """DB::IngestExternalFile for sorted (key, value) pairs (see rocksplicator_b200/sst.py for SST files);
+        behind=True: IngestExternalFileOptions::ingest_behind (allow_global_seqno plays no part)"""
         n = len(sorted_kv)
         koff = np.zeros(n + 1, dtype=np.uint64)
         voff = np.zeros(n + 1, dtype=np.uint64)
@@ -397,6 +413,8 @@ class Shard:
         np.cumsum(np.fromiter((len(v) for _, v in sorted_kv), dtype=np.uint64, count=n), out=voff[1:])
         keys = b"".join(k for k, _ in sorted_kv) + b"\0"
         vals = b"".join(v for _, v in sorted_kv) + b"\0"
+        if behind:
+            return self.lib.rsp_ingest_sorted_behind(self.h, n, keys, koff.ctypes.data, vals, voff.ctypes.data)
         return self.lib.rsp_ingest_sorted(self.h, n, keys, koff.ctypes.data, vals, voff.ctypes.data,
                                           1 if allow_global_seqno else 0, None)
 

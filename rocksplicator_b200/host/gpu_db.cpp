@@ -61,7 +61,8 @@ Status GpuDB::Open(const rocksdb::Options& options, const std::string& name, roc
     else { so.merge_op = RSP_MERGE_CALLBACK; so.merge_fn = &GpuDB::MergeTrampoline; so.merge_state = options.merge_operator.get(); }
   }
   rsp_shard* sh = nullptr;
-  const int rc = rsp_shard_open(engine->raw(), name.c_str(), &so, &sh);
+  const int rc = rsp_shard_open_ex(engine->raw(), name.c_str(), &so,
+                                   options.allow_ingest_behind ? RSP_SHARD_ALLOW_INGEST_BEHIND : 0u, &sh);
   if (rc != RSP_OK) return rc == RSP_INVALID_ARGUMENT ? Status::InvalidArgument("db already open: " + name) : Status::IOError("rsp_shard_open");
   GpuDB* db = new GpuDB();
   db->name_ = name;
@@ -223,8 +224,12 @@ Status GpuDB::IngestExternalFile(const std::vector<std::string>& files, const ro
   keys.push_back('\0');
   vals.push_back('\0');
   std::lock_guard<std::mutex> g(write_mu_);
-  const int rc = rsp_ingest_sorted(shard_, koff.size() - 1, (const uint8_t*)keys.data(), koff.data(), (const uint8_t*)vals.data(),
-                                   voff.data(), opt.allow_global_seqno ? 1 : 0, nullptr);
+  // ingest_behind: the file goes to the shard's ingested-behind tier; allow_global_seqno plays no part
+  const int rc = opt.ingest_behind
+      ? rsp_ingest_sorted_behind(shard_, koff.size() - 1, (const uint8_t*)keys.data(), koff.data(), (const uint8_t*)vals.data(),
+                                 voff.data())
+      : rsp_ingest_sorted(shard_, koff.size() - 1, (const uint8_t*)keys.data(), koff.data(), (const uint8_t*)vals.data(),
+                          voff.data(), opt.allow_global_seqno ? 1 : 0, nullptr);
   if (rc != RSP_OK) return ToStatus(rc);
   if (opt.move_files)
     for (const auto& f : files) remove(f.c_str());  // the data now lives in HBM; a moved file is gone from its old place
@@ -554,9 +559,10 @@ rocksdb::Iterator* GpuDB::NewIterator(const rocksdb::ReadOptions& o) {
   return new GpuIterator(it);
 }
 
-Status GpuDB::CompactRange(const rocksdb::CompactRangeOptions&, const Slice* begin, const Slice* end) {
+Status GpuDB::CompactRange(const rocksdb::CompactRangeOptions& o, const Slice* begin, const Slice* end) {
   if (begin || end) return Status::NotSupported("partial CompactRange");  // the reference passes (nullptr, nullptr)
-  return ToStatus(rsp_compact(shard_));
+  // change_level: the ingested-behind tier is folded in too (change_level = false leaves it at the bottom level)
+  return ToStatus(rsp_compact_ex(shard_, o.change_level ? RSP_COMPACT_CHANGE_LEVEL : 0u));
 }
 Status GpuDB::Flush(const rocksdb::FlushOptions&) { return ToStatus(rsp_flush(shard_)); }
 rocksdb::SequenceNumber GpuDB::GetLatestSequenceNumber() const { return rsp_latest_seq(shard_); }
@@ -631,12 +637,17 @@ bool GpuDB::GetProperty(const Slice& property, std::string* value) {
 }
 
 void GpuDB::GetColumnFamilyMetaData(rocksdb::ColumnFamilyMetaData* meta) {
-  // the newest runs play level 0, the oldest (fully merged) run the bottom level
+  // the newest runs play level 0, the oldest (fully merged) run the bottom level.  With allow_ingest_behind the bottom
+  // level is the ingested-behind tier alone and every other run sits at level 0 (RocksDB keeps Lmax for those files).
   rsp_stats st;
   rsp_get_stats(shard_, &st);
   meta->levels.clear();
   for (int l = 0; l < options_.num_levels; l++) meta->levels.push_back({l, 0});
-  if (st.n_runs == 1) meta->levels.back().size = st.run_bytes;
+  if (options_.allow_ingest_behind) {
+    const uint64_t behind = rsp_shard_behind_bytes(shard_);
+    meta->levels.back().size = behind;
+    meta->levels[0].size += st.run_bytes - behind;
+  } else if (st.n_runs == 1) meta->levels.back().size = st.run_bytes;
   else if (st.n_runs > 1) { meta->levels[0].size = st.run_bytes / 2; meta->levels.back().size = st.run_bytes - st.run_bytes / 2; }
   meta->size = st.run_bytes;
   meta->file_count = st.n_runs;

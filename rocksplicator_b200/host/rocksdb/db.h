@@ -57,6 +57,7 @@ class DB {
   virtual Status GetUpdatesSince(SequenceNumber seq, std::unique_ptr<TransactionLogIterator>* iter) = 0;
   virtual ColumnFamilyHandle* DefaultColumnFamily() const = 0;
   virtual Options GetOptions() const = 0;
+  virtual DBOptions GetDBOptions() const { return GetOptions(); }
   virtual bool GetProperty(const Slice& property, std::string* value) = 0;
   virtual int NumberLevels() = 0;
   virtual void GetColumnFamilyMetaData(ColumnFamilyMetaData* meta) = 0;

@@ -26,8 +26,15 @@ struct IngestExternalFileOptions {
   bool snapshot_consistency = true;
   bool allow_global_seqno = true;
   bool allow_blocking_flush = true;
+  // RocksDB 5.7: the file goes below everything the DB holds (needs DBOptions::allow_ingest_behind)
+  bool ingest_behind = false;
 };
-struct Options {
+// admin_handler.cpp:1669-1688 reads allow_ingest_behind through DB::GetDBOptions()
+struct DBOptions {
+  // keep the bottom level for files ingested behind: no compaction is bottom-most, tombstones are never dropped
+  bool allow_ingest_behind = false;
+};
+struct Options : DBOptions {
   bool create_if_missing = false;
   bool error_if_exists = false;
   size_t write_buffer_size = 64 << 20;
