@@ -75,8 +75,8 @@ struct Arena {
     in_use += c;
     return (void*)it->first;
   }
-  void release(void* p, size_t n) {
-    (void)n;
+  // (the block map knows every block's size: a size passed by a caller is not needed and not read)
+  void release(void* p, size_t /*unused*/ = 0) {
     if (!p) return;
 #ifdef RSP_EMUL
     if (exact()) { slab_free(p); return; }
@@ -140,6 +140,36 @@ struct Arena {
     free_by_size.clear();
     in_use = reserved = free_bytes = 0;
   }
+};
+
+// One arena block and the duty to give it back: released when the handle is destroyed or assigned over, handed on by
+// move.  An empty handle owns nothing and its get() is null.
+class ArenaBlock {
+ public:
+  ArenaBlock() = default;
+  ArenaBlock(Arena& a, size_t n) : a_(&a), p_(a.alloc(n)) {}
+  ArenaBlock(ArenaBlock&& o) noexcept : a_(o.a_), p_(o.p_) { o.p_ = nullptr; }
+  ArenaBlock& operator=(ArenaBlock&& o) noexcept {
+    if (this != &o) {
+      reset();
+      a_ = o.a_;
+      p_ = o.p_;
+      o.p_ = nullptr;
+    }
+    return *this;
+  }
+  ~ArenaBlock() { reset(); }
+  template <class T = void>
+  T* get() const { return static_cast<T*>(p_); }
+  explicit operator bool() const { return p_ != nullptr; }
+  void reset() {
+    if (p_) a_->release(p_);
+    p_ = nullptr;
+  }
+
+ private:
+  Arena* a_ = nullptr;
+  void* p_ = nullptr;
 };
 
 }  // namespace rsp

@@ -103,44 +103,42 @@ static void* arena_slab_alloc(size_t n) {
 }
 static void arena_slab_free(void* p) { cudaFree(p); }
 
-// growable device / pinned scratch
-struct DevBuf {
+// growable scratch over an allocate / free pair.  Growth is all or nothing: the old buffer is gone before the new one is
+// asked for, so a failed request leaves the buffer empty rather than a freed pointer behind a larger capacity
+inline cudaError_t dev_alloc(void** p, size_t n) { return cudaMalloc(p, n); }
+inline cudaError_t pin_alloc(void** p, size_t n) { return cudaHostAlloc(p, n, cudaHostAllocDefault); }
+template <cudaError_t (*Alloc)(void**, size_t), cudaError_t (*Free)(void*)>
+struct GrowBuf {
   void* p = nullptr;
   size_t cap = 0;
+  GrowBuf() = default;
+  GrowBuf(const GrowBuf&) = delete;
+  GrowBuf& operator=(const GrowBuf&) = delete;
+  ~GrowBuf() { destroy(); }
   void* get(size_t n) {
     if (n > cap) {
-      if (p) CUDA_OK(cudaFree(p));
-      cap = std::max(n, cap * 2);
-      CUDA_OK(cudaMalloc(&p, cap));
+      const size_t want = std::max(n, cap * 2);
+      destroy();
+      CUDA_OK(Alloc(&p, want));
+      cap = want;
     }
     return p;
   }
-  void destroy() { if (p) cudaFree(p); p = nullptr; cap = 0; }
-};
-struct PinBuf {
-  void* p = nullptr;
-  size_t cap = 0;
-  void* get(size_t n) {
-    if (n > cap) {
-      if (p) CUDA_OK(cudaFreeHost(p));
-      cap = std::max(n, cap * 2);
-      CUDA_OK(cudaHostAlloc(&p, cap, cudaHostAllocDefault));
-    }
-    return p;
+  void destroy() {
+    if (p) Free(p);
+    p = nullptr;
+    cap = 0;
   }
-  void destroy() { if (p) cudaFreeHost(p); p = nullptr; cap = 0; }
 };
+using DevBuf = GrowBuf<dev_alloc, cudaFree>;
+using PinBuf = GrowBuf<pin_alloc, cudaFreeHost>;
 
 // ------------------------------------------------------------------------------------------------
 // the block index is staged by one TMA bulk copy, whose size is a multiple of 16 bytes (k_read.cu run_lower_bound_warp)
 static inline size_t blk_pfx_bytes(u32 n_blocks) { return ((size_t)n_blocks * 8 + 15) & ~(size_t)15; }
 
 struct Run {
-  Arena* arena;
-  u8* heap = nullptr;
-  u32* ent_off = nullptr;
-  u32* hslots = nullptr;
-  u64* blk_pfx = nullptr;
+  ArenaBlock heap, ent_off, hslots, blk_pfx;
   u32 n_ent = 0, heap_units = 0, n_buckets = 0, ord_bits = 0, uniform_units = 0, n_blocks = 0, flags = 0, kv_len = 0;
   // host-only: behind = the run belongs to the ingested-behind tier of an allow-ingest-behind shard (the oldest runs,
   // key-disjoint, all at sequence 0); seq0 = the run holds sequence-0 data (an ingest that took no global sequence
@@ -151,18 +149,17 @@ struct Run {
   std::vector<std::pair<std::string, std::string>> file_ranges;
   RunDev dev() const {
     RunDev r;
-    r.heap = heap; r.ent_off = ent_off; r.hslots = hslots; r.blk_pfx = blk_pfx;
+    r.heap = heap.get<u8>(); r.ent_off = ent_off.get<u32>(); r.hslots = hslots.get<u32>(); r.blk_pfx = blk_pfx.get<u64>();
     r.n_ent = n_ent; r.n_buckets = n_buckets; r.ord_bits = ord_bits; r.uniform_units = uniform_units;
     r.n_blocks = n_blocks; r.heap_units = heap_units; r.flags = flags; r.kv_len = kv_len;
     return r;
   }
   size_t bytes() const { return (size_t)heap_units * 16; }
-  ~Run() {
-    arena->release(heap, (size_t)heap_units * 16);
-    arena->release(ent_off, (size_t)n_ent * 4);
-    arena->release(hslots, (size_t)n_buckets * RUN_BUCKET_SLOTS * 4);
-    arena->release(blk_pfx, blk_pfx_bytes(n_blocks));
-  }
+};
+
+// a shard's memtable buffers; ShardDev::mt_* is their device-side description
+struct Memtable {
+  ArenaBlock heap, slots, ent_off;
 };
 
 struct rsp_engine;
@@ -182,7 +179,7 @@ struct rsp_shard {
   std::string last_error;
   std::mutex err_mu;
   rsp_stats stats{};
-  size_t mt_heap_bytes = 0, mt_slot_bytes = 0, mt_ent_bytes = 0;
+  Memtable mt;
   bool counted_multirun = false;  // this shard is counted in the engine's n_multirun
   bool merging = false;           // a background merge of runs [bg_first_pinned ..] is in flight
   u64 uid = 0;                    // never reused: a background merge recognises the shard it planned for
@@ -219,7 +216,6 @@ struct rsp_staged {
   std::vector<rsp_shard*> group_shard;
   std::vector<u32> need_units, need_ents;
   void* dev = nullptr;          // device image
-  size_t dev_bytes = 0;
   TickDev tick{};
   cudaStream_t last_stream = nullptr;
   size_t res_bytes = 0;         // gres + per-batch status words, contiguous
@@ -288,7 +284,6 @@ struct rsp_engine {
   std::atomic<u32> n_string_append{0};
   struct Compactor* compactor = nullptr;
   u32 mg_parity = 0;
-  size_t pending_cap = 0;
   // where the last host-form or device-form MultiGet left its deferred lookups (rsp_debug_last_pending): the
   // 16-byte-key kernel ran (fast), the counter parity of a device-form launch, or the chunking of a host-form call
   struct {
@@ -334,7 +329,7 @@ static void describe_shard(rsp_engine* e, rsp_shard* s, ShardFast* f_out, ShardF
     else memset(&s->h.runs[i], 0, sizeof(RunDev));
   }
   auto describe = [](const Run& r, ShardFast* f) {
-    f->run0_heap = (u64)r.heap; f->run0_hslots = (u64)r.hslots; f->n_buckets = r.n_buckets;
+    f->run0_heap = (u64)r.heap.get(); f->run0_hslots = (u64)r.hslots.get(); f->n_buckets = r.n_buckets;
     f->meta = r.ord_bits | (std::min<u32>(r.uniform_units, 255u) << FAST_META_UNITS_SHIFT);
   };
   ShardFast f;
@@ -370,15 +365,21 @@ static void stage_upload(rsp_engine* e, rsp_shard* s, bool runs_only, bool zero_
   u.index = s->index; u.runs_only = runs_only ? 1u : 0u; u.zero_mt = zero_mt ? 1u : 0u; u.pad = 0;
   u.sd = s->h;
 }
+// Staging for n upload records, taken before a caller changes any shard: a commit of at most n records after that
+// allocates nothing, so it cannot leave the host mirrors ahead of the device for want of memory.
+static void reserve_uploads(rsp_engine* e, size_t n) {
+  if (e->up_ev_recorded) CUDA_OK(cudaEventSynchronize(e->up_ev));  // the staging buffers of the previous batch
+  e->pin_up.get(n * sizeof(ShardUpload));
+  e->dev_up.get(n * sizeof(ShardUpload));
+}
 static void commit_uploads(rsp_engine* e, UploadBatch* b) {
   const size_t n = b->recs.size();
   if (!n) return;
   const size_t bytes = n * sizeof(ShardUpload);
-  if (e->up_ev_recorded) CUDA_OK(cudaEventSynchronize(e->up_ev));  // the staging buffers of the previous batch
-  void* pin = e->pin_up.get(bytes);
-  memcpy(pin, b->recs.data(), bytes);
-  ShardUpload* d_up = (ShardUpload*)e->dev_up.get(bytes);
-  CUDA_OK(cudaMemcpyAsync(d_up, pin, bytes, cudaMemcpyHostToDevice, e->st));
+  reserve_uploads(e, n);
+  memcpy(e->pin_up.p, b->recs.data(), bytes);
+  ShardUpload* d_up = (ShardUpload*)e->dev_up.p;
+  CUDA_OK(cudaMemcpyAsync(d_up, e->pin_up.p, bytes, cudaMemcpyHostToDevice, e->st));
   launch_upload_shards(d_up, (u32)n, e->d_shards, e->d_fast, e->d_fast_runs, e->d_mt_filter, e->st);
   CUDA_OK(cudaGetLastError());
   CUDA_OK(cudaEventRecord(e->up_ev, e->st));
@@ -394,25 +395,22 @@ static u32 next_pow2(u32 x) {
 }
 
 // (re)allocate an empty memtable able to hold at least `units` heap units and `ents` entries; the caller installs it
-// with a zero_mt upload record, which clears its slot table and filter row
+// with a zero_mt upload record, which clears its slot table and filter row.  The new buffers are taken while the old
+// ones are still held, so a failed allocation leaves the old memtable installed and whole.
 static void alloc_memtable(rsp_engine* e, rsp_shard* s, u64 units, u64 ents) {
   Arena& a = e->arena;
-  if (s->h.mt_heap) {
-    wait_readers(e);
-    CUDA_OK(cudaStreamSynchronize(e->st));  // nothing may still read the buffers being recycled
-    a.release(s->h.mt_heap, s->mt_heap_bytes);
-    a.release(s->h.mt_slots, s->mt_slot_bytes);
-    a.release(s->h.mt_ent_off, s->mt_ent_bytes);
-  }
   u64 want_units = std::max<u64>(units, (s->opts.write_buffer_bytes ? s->opts.write_buffer_bytes : (1u << 20)) / 16);
   u64 want_ents = std::max<u64>(ents, want_units / 7);  // a 16 B/64 B Put is 7 units
   u32 slot_cap = next_pow2((u32)std::max<u64>(16, want_ents * 2));  // (k_upload_shards clears >= 16 slots)
-  s->mt_heap_bytes = want_units * 16;
-  s->mt_slot_bytes = (size_t)slot_cap * 8;
-  s->mt_ent_bytes = want_ents * 4;
-  s->h.mt_heap = (u8*)a.alloc(s->mt_heap_bytes);
-  s->h.mt_slots = (u64*)a.alloc(s->mt_slot_bytes);
-  s->h.mt_ent_off = (u32*)a.alloc(s->mt_ent_bytes);
+  Memtable mt{ArenaBlock(a, want_units * 16), ArenaBlock(a, (size_t)slot_cap * 8), ArenaBlock(a, want_ents * 4)};
+  if (s->mt.heap) {
+    wait_readers(e);
+    CUDA_OK(cudaStreamSynchronize(e->st));  // nothing may still read the buffers being let go
+  }
+  s->mt = std::move(mt);
+  s->h.mt_heap = s->mt.heap.get<u8>();
+  s->h.mt_slots = s->mt.slots.get<u64>();
+  s->h.mt_ent_off = s->mt.ent_off.get<u32>();
   s->h.mt_slot_mask = slot_cap - 1;
   s->h.mt_heap_cap = (u32)want_units;
   s->h.mt_ent_cap = (u32)want_ents;
@@ -431,16 +429,17 @@ struct JobHost {
   bool has_mem;     // the memtable is a source (flush)
   size_t n_merged;  // srcs.size(): the runs replaced by the output
   std::vector<std::shared_ptr<Run>> srcs;
-  size_t items_b, items2_b, coranks_b, keep_b, fold_b;
+  ArenaBlock items, items2, coranks, keep_units, out_pos, out_ord, fold_val;  // the job's work buffers
   bool generic_sort = false;  // the memtable took the comparison sort (k_flush_sort left it: totals[7])
 };
-// one batch of flush / merge jobs: planned under the engine mutex, run on a stream, installed under the mutex again
+// one batch of flush / merge jobs: planned under the engine mutex, run on a stream, installed under the mutex again.
+// A plan is only destroyed with its stream idle (run_jobs sees to that when it fails), so its buffers go back then.
 struct CompactPlan {
   std::vector<JobHost> jh;
   std::vector<CompactJob> jobs;
   std::vector<std::shared_ptr<Run>> outs;
-  CompactJob* d_jobs = nullptr;
-  u32* d_totals = nullptr;  // [8 x jobs], contiguous: one copy brings every job's sizes back
+  ArenaBlock d_jobs;
+  ArenaBlock d_totals;  // [8 x jobs], contiguous: one copy brings every job's sizes back
   float ms = 0;
 };
 enum CompactMode {
@@ -481,34 +480,22 @@ static size_t unpinned_runs(const rsp_shard* s) {
 
 static void bg_request(rsp_engine* e, rsp_shard* s);
 
-// the work buffers of a job whose sources are set (n_src, src_n, seg_start, n_items, items_len, n_tiles)
-// (out of device memory: the buffers taken so far go back to the arena before the exception leaves)
+// the work buffers of a job whose sources are set (n_src, src_n, seg_start, n_items, items_len, n_tiles), owned by `h`
 static void alloc_job_work(Arena& a, CompactJob* j, JobHost* h) {
   const u32 ns = j->n_src;
-  h->items_b = (size_t)std::max<u32>(1, j->items_len) * sizeof(SortItem);
-  h->items2_b = ns > 1 ? (size_t)std::max<u32>(1, j->n_items) * sizeof(SortItem) : 0;
-  h->coranks_b = ns > 1 ? (size_t)(j->n_tiles + 1) * ns * 4 : 0;
-  h->keep_b = (size_t)std::max<u32>(1, j->n_items) * 4;
-  h->fold_b = (size_t)std::max<u32>(1, j->n_items) * 8;
-  j->items = nullptr; j->items2 = nullptr; j->coranks = nullptr;
-  j->keep_units = nullptr; j->out_pos = nullptr; j->out_ord = nullptr; j->fold_val = nullptr;
-  try {
-    j->items = (SortItem*)a.alloc(h->items_b);
-    j->items2 = ns > 1 ? (SortItem*)a.alloc(h->items2_b) : nullptr;
-    j->coranks = ns > 1 ? (u32*)a.alloc(h->coranks_b) : nullptr;
-    j->keep_units = (u32*)a.alloc(h->keep_b);
-    j->out_pos = (u32*)a.alloc(h->keep_b);
-    j->out_ord = (u32*)a.alloc(h->keep_b);
-    j->fold_val = (u64*)a.alloc(h->fold_b);
-  } catch (...) {
-    if (j->items) a.release(j->items, h->items_b);
-    if (j->items2) a.release(j->items2, h->items2_b);
-    if (j->coranks) a.release(j->coranks, h->coranks_b);
-    if (j->keep_units) a.release(j->keep_units, h->keep_b);
-    if (j->out_pos) a.release(j->out_pos, h->keep_b);
-    if (j->out_ord) a.release(j->out_ord, h->keep_b);
-    throw;
+  const size_t n = std::max<u32>(1, j->n_items);
+  h->items = ArenaBlock(a, (size_t)std::max<u32>(1, j->items_len) * sizeof(SortItem));
+  if (ns > 1) {
+    h->items2 = ArenaBlock(a, n * sizeof(SortItem));
+    h->coranks = ArenaBlock(a, (size_t)(j->n_tiles + 1) * ns * 4);
   }
+  h->keep_units = ArenaBlock(a, n * 4);
+  h->out_pos = ArenaBlock(a, n * 4);
+  h->out_ord = ArenaBlock(a, n * 4);
+  h->fold_val = ArenaBlock(a, n * 8);
+  j->items = h->items.get<SortItem>(); j->items2 = h->items2.get<SortItem>(); j->coranks = h->coranks.get<u32>();
+  j->keep_units = h->keep_units.get<u32>(); j->out_pos = h->out_pos.get<u32>(); j->out_ord = h->out_ord.get<u32>();
+  j->fold_val = h->fold_val.get<u64>();
   j->sorted = ns > 1 ? j->items2 : j->items;
 }
 
@@ -542,7 +529,7 @@ static void plan_jobs(rsp_engine* e, const std::vector<rsp_shard*>& shards, Comp
     }
     CompactJob j;
     memset(&j, 0, sizeof(j));
-    JobHost h{s, s->index, s->uid, full, has_mem, n_merged, {}, 0, 0, 0, 0, 0};
+    JobHost h{s, s->index, s->uid, full, has_mem, n_merged, {}};
     u32 ns = 0;
     if (has_mem) {
       j.src_heap[ns] = s->h.mt_heap; j.src_ent_off[ns] = s->h.mt_ent_off; j.src_n[ns] = s->h.mt_count;
@@ -551,7 +538,7 @@ static void plan_jobs(rsp_engine* e, const std::vector<rsp_shard*>& shards, Comp
     }
     for (size_t r = first; r < first + n_merged; r++) {
       auto& run = s->runs[r];
-      j.src_heap[ns] = run->heap; j.src_ent_off[ns] = run->ent_off; j.src_n[ns] = run->n_ent; j.src_is_mem[ns] = 0;
+      j.src_heap[ns] = run->heap.get<u8>(); j.src_ent_off[ns] = run->ent_off.get<u32>(); j.src_n[ns] = run->n_ent; j.src_is_mem[ns] = 0;
       ns++;
       h.srcs.push_back(run);
     }
@@ -573,21 +560,23 @@ static void plan_jobs(rsp_engine* e, const std::vector<rsp_shard*>& shards, Comp
       s->merging = true;
       s->bg_first_pinned = h.srcs.front().get();
     }
-    plan->jh.push_back(h);
+    plan->jh.push_back(std::move(h));
     plan->jobs.push_back(j);
   }
 }
 
 // ---- run (no engine mutex needed: sources are pinned, outputs are private until installed) -----------------
-static void run_jobs(rsp_engine* e, CompactPlan* plan, cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1, PinBuf* pin_totals) {
+// On failure the stream is synchronised before the exception leaves, so that the plan's buffers can go back.
+static void run_jobs(rsp_engine* e, CompactPlan* plan, cudaStream_t st, cudaEvent_t ev0, cudaEvent_t ev1,
+                     PinBuf* pin_totals) try {
   Arena& a = e->arena;
   std::vector<CompactJob>& jobs = plan->jobs;
   const u32 nj = (u32)jobs.size();
-  plan->d_jobs = (CompactJob*)a.alloc(sizeof(CompactJob) * nj);
-  plan->d_totals = (u32*)a.alloc((size_t)32 * nj);
-  for (u32 i = 0; i < nj; i++) jobs[i].totals = plan->d_totals + 8 * (size_t)i;
-  CUDA_OK(cudaMemsetAsync(plan->d_totals, 0, (size_t)32 * nj, st));
-  CompactJob* d_jobs = plan->d_jobs;
+  plan->d_jobs = ArenaBlock(a, sizeof(CompactJob) * nj);
+  plan->d_totals = ArenaBlock(a, (size_t)32 * nj);
+  for (u32 i = 0; i < nj; i++) jobs[i].totals = plan->d_totals.get<u32>() + 8 * (size_t)i;
+  CUDA_OK(cudaMemsetAsync(plan->d_totals.get(), 0, (size_t)32 * nj, st));
+  CompactJob* d_jobs = plan->d_jobs.get<CompactJob>();
   CUDA_OK(cudaMemcpyAsync(d_jobs, jobs.data(), sizeof(CompactJob) * nj, cudaMemcpyHostToDevice, st));
   CUDA_OK(cudaEventRecord(ev0, st));
   launch_compact_sort(d_jobs, jobs.data(), nj, st);
@@ -596,7 +585,7 @@ static void run_jobs(rsp_engine* e, CompactPlan* plan, cudaStream_t st, cudaEven
   e->launches += 5;
   // the sizing round trip: ONE copy into pinned memory (r02 issued a 32-byte pageable copy per job)
   const u32* totals = (const u32*)pin_totals->get((size_t)32 * nj);
-  CUDA_OK(cudaMemcpyAsync((void*)totals, plan->d_totals, (size_t)32 * nj, cudaMemcpyDeviceToHost, st));
+  CUDA_OK(cudaMemcpyAsync((void*)totals, plan->d_totals.get(), (size_t)32 * nj, cudaMemcpyDeviceToHost, st));
   CUDA_OK(cudaStreamSynchronize(st));
   u32 max_items = 0, max_buckets = 0;
   plan->outs.resize(nj);
@@ -606,7 +595,6 @@ static void run_jobs(rsp_engine* e, CompactPlan* plan, cudaStream_t st, cudaEven
     const u32 non_put = totals[8 * i + 4], kvmin = totals[8 * i + 5], kvmax = totals[8 * i + 6];
     plan->jh[i].generic_sort = totals[8 * i + 7] != 0;
     auto r = std::make_shared<Run>();
-    r->arena = &a;
     r->n_ent = ents; r->heap_units = units; r->uniform_units = uni;
     if (ents && uni && non_put == 0 && kvmin == kvmax) { r->flags = RUN_ALL_PUT_FIXED; r->kv_len = kvmin; }
     r->n_blocks = (ents + RSP_BLOCK_ENTRIES - 1) / RSP_BLOCK_ENTRIES;
@@ -615,12 +603,13 @@ static void run_jobs(rsp_engine* e, CompactPlan* plan, cudaStream_t st, cudaEven
     r->n_buckets = std::max<u32>(1, (u32)(((u64)keys + 3) / 4));
     r->ord_bits = 1;
     while ((1ull << r->ord_bits) <= ents) r->ord_bits++;
-    r->heap = (u8*)a.alloc((size_t)units * 16);
-    r->ent_off = (u32*)a.alloc((size_t)ents * 4);
-    r->hslots = (u32*)a.alloc((size_t)r->n_buckets * RUN_BUCKET_SLOTS * 4);
-    r->blk_pfx = (u64*)a.alloc(blk_pfx_bytes(r->n_blocks));
+    r->heap = ArenaBlock(a, (size_t)units * 16);
+    r->ent_off = ArenaBlock(a, (size_t)ents * 4);
+    r->hslots = ArenaBlock(a, (size_t)r->n_buckets * RUN_BUCKET_SLOTS * 4);
+    r->blk_pfx = ArenaBlock(a, blk_pfx_bytes(r->n_blocks));
     max_buckets = std::max(max_buckets, r->n_buckets);
-    j.out_heap = r->heap; j.out_ent_off = r->ent_off; j.out_hslots = r->hslots; j.out_blk_pfx = r->blk_pfx;
+    j.out_heap = r->heap.get<u8>(); j.out_ent_off = r->ent_off.get<u32>(); j.out_hslots = r->hslots.get<u32>();
+    j.out_blk_pfx = r->blk_pfx.get<u64>();
     j.out_n_buckets = r->n_buckets; j.out_ord_bits = r->ord_bits;
     plan->outs[i] = r;
     max_items = std::max(max_items, j.n_items);
@@ -633,25 +622,9 @@ static void run_jobs(rsp_engine* e, CompactPlan* plan, cudaStream_t st, cudaEven
   CUDA_OK(cudaEventRecord(ev1, st));
   CUDA_OK(cudaStreamSynchronize(st));
   cudaEventElapsedTime(&plan->ms, ev0, ev1);
-}
-
-static void release_work(rsp_engine* e, CompactPlan* plan) {
-  Arena& a = e->arena;
-  for (size_t i = 0; i < plan->jobs.size(); i++) {
-    const CompactJob& j = plan->jobs[i];
-    const JobHost& h = plan->jh[i];
-    a.release(j.items, h.items_b);
-    if (j.items2) a.release(j.items2, h.items2_b);
-    if (j.coranks) a.release(j.coranks, h.coranks_b);
-    a.release(j.keep_units, h.keep_b);
-    a.release(j.out_pos, h.keep_b);
-    a.release(j.out_ord, h.keep_b);
-    a.release(j.fold_val, h.fold_b);
-  }
-  if (plan->d_jobs) a.release(plan->d_jobs, sizeof(CompactJob) * plan->jobs.size());
-  if (plan->d_totals) a.release(plan->d_totals, (size_t)32 * plan->jobs.size());
-  plan->d_jobs = nullptr;
-  plan->d_totals = nullptr;
+} catch (...) {
+  cudaStreamSynchronize(st);
+  throw;
 }
 
 // ---- install (engine mutex held): the new run takes the place of its sources in the shard's run list; readers keep
@@ -659,6 +632,7 @@ static void release_work(rsp_engine* e, CompactPlan* plan) {
 static void install_jobs(rsp_engine* e, CompactPlan* plan, CompactMode mode) {
   const u32 nj = (u32)plan->jobs.size();
   if (mode == COMPACT_MERGE) wait_readers(e);  // (the foreground path did this before it touched a memtable)
+  reserve_uploads(e, nj);  // nothing below fails half-way: the shards and their descriptors change together
   UploadBatch up;
   up.recs.reserve(nj);
   for (u32 i = 0; i < nj; i++) {
@@ -718,23 +692,11 @@ static void install_jobs(rsp_engine* e, CompactPlan* plan, CompactMode mode) {
 // (engine mutex held throughout)
 static void compact_shards(rsp_engine* e, const std::vector<rsp_shard*>& shards, CompactMode mode) {
   CompactPlan plan;
-  try {
-    plan_jobs(e, shards, mode, &plan);
-  } catch (...) {  // the work buffers of the jobs planned so far go back
-    release_work(e, &plan);
-    throw;
-  }
+  plan_jobs(e, shards, mode, &plan);
   if (plan.jobs.empty()) return;
   wait_readers(e);
-  try {
-    run_jobs(e, &plan, e->st, e->ev0, e->ev1, &e->pin_totals);
-  } catch (...) {  // (out of device memory, typically): nothing was installed; the work buffers and partial outputs go back
-    cudaStreamSynchronize(e->st);
-    release_work(e, &plan);
-    throw;
-  }
+  run_jobs(e, &plan, e->st, e->ev0, e->ev1, &e->pin_totals);
   install_jobs(e, &plan, mode);
-  release_work(e, &plan);
 }
 
 // the memtable's contents as a private sorted run (an iterator's snapshot): nothing about the shard changes
@@ -742,14 +704,7 @@ static std::shared_ptr<Run> snapshot_memtable(rsp_engine* e, rsp_shard* s) {
   CompactPlan plan;
   plan_jobs(e, {s}, COMPACT_SNAPSHOT, &plan);
   if (plan.jobs.empty()) return nullptr;
-  try {
-    run_jobs(e, &plan, e->st, e->ev0, e->ev1, &e->pin_totals);
-  } catch (...) {
-    cudaStreamSynchronize(e->st);
-    release_work(e, &plan);
-    throw;
-  }
-  release_work(e, &plan);
+  run_jobs(e, &plan, e->st, e->ev0, e->ev1, &e->pin_totals);
   s->stats.compaction_bytes_read += (u64)s->h.mt_tail * 16;
   return plan.outs[0]->n_ent ? plan.outs[0] : nullptr;
 }
@@ -852,15 +807,11 @@ void Compactor::loop() {
           cudaSetDevice(e->device);
           install_jobs(e, &plan, COMPACT_MERGE);
         }
-        release_work(e, &plan);
       } catch (...) {
-        abi_caught();  // a CUDA failure: recorded; the shards keep their runs, the work buffers go back
-        cudaStreamSynchronize(stream);
+        abi_caught();  // a CUDA failure: recorded; the shards keep their runs, the plan's buffers go back with it
         std::lock_guard<std::mutex> g(e->mu);
         for (JobHost& h : plan.jh)
           if (h.s && h.index < e->slots.size() && e->slots[h.index] == h.s && h.s->uid == h.uid) { h.s->merging = false; h.s->bg_first_pinned = nullptr; }
-        release_work(e, &plan);
-        plan.outs.clear();
       }
     }
   }
@@ -1054,7 +1005,6 @@ static int stage_build(rsp_engine* e, size_t n, const uint32_t* shard_ix, const 
   u8* dev;
   if (own_dev) {
     CUDA_OK(cudaMalloc(&sg->dev, dev_b));
-    sg->dev_bytes = dev_b;
     dev = (u8*)sg->dev;
   } else {
     dev = (u8*)e->dev_tick.get(dev_b);
@@ -1131,12 +1081,13 @@ static int reserve_for(rsp_engine* e, const rsp_staged* sg) {
       rsp_shard* s = sg->group_shard[g];
       const u64 nu = sg->need_units[g], ne = sg->need_ents[g];
       if (!fits(s, nu, ne)) {  // empty but too small for this tick
+        if (up.recs.empty()) reserve_uploads(e, sg->group_shard.size() - g);
         alloc_memtable(e, s, nu + nu / 2, ne + ne / 2);
         stage_upload(e, s, false, true, &up);
         did_work = true;
       }
     }
-  } catch (...) {  // (out of device memory): the memtables re-sized so far are installed all the same
+  } catch (...) {  // (out of device memory): the memtables re-sized so far are installed all the same (staging reserved)
     commit_uploads(e, &up);
     throw;
   }
@@ -1465,11 +1416,9 @@ static void pending_mark(rsp_engine* e, cudaStream_t stream) {
 }
 static void set_pending(rsp_engine* e, GetArgs& a, size_t n, cudaStream_t stream) {
   pending_order(e, stream);
-  if ((n + 8) * 4 > e->pending_cap) {
+  if ((n + 8) * 4 > e->dev_pending.cap) {
     if (e->pending_ev_recorded) CUDA_OK(cudaEventSynchronize(e->pending_ev));  // the old list may still be read
-    e->pending_cap = std::max<size_t>((n + 8) * 4, e->pending_cap * 2);
-    u32* p = (u32*)e->dev_pending.get(e->pending_cap);
-    CUDA_OK(cudaMemsetAsync(p, 0, 16, stream));
+    CUDA_OK(cudaMemsetAsync(e->dev_pending.get((n + 8) * 4), 0, 16, stream));
     e->mg_parity = 0;
   }
   a.n_special = (u32*)e->dev_pending.p;
@@ -1545,11 +1494,7 @@ static int multi_get_locked(rsp_engine* e, size_t n, const uint32_t* shard_ix, c
     CUDA_OK(cudaEventSynchronize(e->pending_ev));  // synchronous anyway
     e->pending_ev_recorded = false;
   }
-  if (scratch_u32 * 4 > e->pending_cap) {
-    e->pending_cap = std::max(scratch_u32 * 4, e->pending_cap * 2);
-    e->dev_pending.get(e->pending_cap);
-  }
-  u32* scratch = (u32*)e->dev_pending.p;
+  u32* scratch = (u32*)e->dev_pending.get(scratch_u32 * 4);
   CUDA_OK(cudaMemsetAsync(scratch, 0, (4 + 2 * n_chunks) * 4, e->st));
   e->mg_parity = 0;
   e->last_mg.fast = false; e->last_mg.host = true; e->last_mg.parity = 0;
@@ -1651,7 +1596,7 @@ static void walk_scan_records(u8* rec, u32 n_out, F f) {
 struct rsp_iter {
   rsp_shard* s;
   std::vector<std::shared_ptr<Run>> pinned;
-  ScanView* d_view = nullptr;
+  ArenaBlock view;  // the ScanView of `pinned`, scanned as a one-entry snapshot table
   struct Ent { std::string first, second; int status; };  // status != 0: the merge of this key failed (empty value)
   std::vector<Ent> buf;
   size_t pos = 0;
@@ -1686,7 +1631,7 @@ static void iter_fetch(rsp_iter* it, const std::string* key, bool exclusive, boo
   for (;;) {
     const u64 koff[2] = {0, key ? key->size() : 0};
     ScanArgs a;
-    a.shards = nullptr; a.views = it->d_view; a.n_views = 1;
+    a.shards = nullptr; a.views = it->view.get<ScanView>(); a.n_views = 1;
     a.flags = SCAN_AT_SLOT | (exclusive ? SCAN_EXCLUSIVE : 0u) | (key ? 0u : SCAN_FROM_EXTREME);
     a.max_entries = (u32)it->want; a.out_stride = it->stride; a.n = 1;
     std::vector<u8> h(it->stride);
@@ -1704,7 +1649,7 @@ static void iter_fetch(rsp_iter* it, const std::string* key, bool exclusive, boo
       if (vl == SCAN_VLEN_HOST_FOLD) {  // operator lives on the host: fold this key against the pinned view
         // (the fold reuses the scan's device scratch: the records are already on the host, in `h`)
         std::string v;
-        const int rc = host_fold_get(e, it->s, (const uint8_t*)k.data(), k.size(), &v, it->d_view);
+        const int rc = host_fold_get(e, it->s, (const uint8_t*)k.data(), k.size(), &v, it->view.get<ScanView>());
         if (rc == RSP_OK) it->buf.push_back({std::move(k), std::move(v), 0});
         else if (rc != RSP_NOT_FOUND) it->buf.push_back({std::move(k), std::string(), rc});
       } else if (vl == SCAN_VLEN_MERGE_FAILED) {
@@ -2135,7 +2080,8 @@ int rsp_engine_create(int device, const rsp_engine_cfg* cfg, rsp_engine** out) {
     const size_t gran = g ? (size_t)atoi(g) : 32;
     if (gran) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, gran);
   }
-  rsp_engine* e = new rsp_engine();
+  // a failure part-way tears down what was built through rsp_engine_destroy
+  std::unique_ptr<rsp_engine, decltype(&rsp_engine_destroy)> e(new rsp_engine(), rsp_engine_destroy);
   e->device = device;
   if (cfg) e->cfg = *cfg;
   if (!e->cfg.max_shards) e->cfg.max_shards = 16384;
@@ -2171,18 +2117,21 @@ int rsp_engine_create(int device, const rsp_engine_cfg* cfg, rsp_engine** out) {
   }
   {
     Compactor* c = new Compactor();
-    c->e = e;
+    c->e = e.get();
     CUDA_OK(cudaStreamCreateWithFlags(&c->stream, cudaStreamNonBlocking));
     CUDA_OK(cudaEventCreate(&c->ev0));
     CUDA_OK(cudaEventCreate(&c->ev1));
     e->compactor = c;
     c->th = std::thread([c] { c->loop(); });
   }
-  *out = e;
+  *out = e.release();
   return RSP_OK;
   } catch (...) { return abi_caught(); }
 }
 
+// (an engine that rsp_engine_create gave up on has null streams and events)
+static void stream_destroy(cudaStream_t s) { if (s) cudaStreamDestroy(s); }
+static void event_destroy(cudaEvent_t ev) { if (ev) cudaEventDestroy(ev); }
 void rsp_engine_destroy(rsp_engine* e) {
   if (!e) return;
   if (Compactor* c = e->compactor) {  // let a merge in flight finish, then stop the thread
@@ -2194,31 +2143,27 @@ void rsp_engine_destroy(rsp_engine* e) {
     c->cv.notify_all();
     if (c->th.joinable()) c->th.join();
     cudaSetDevice(e->device);
-    cudaStreamDestroy(c->stream);
-    cudaEventDestroy(c->ev0);
-    cudaEventDestroy(c->ev1);
-    c->pin_totals.destroy();
+    stream_destroy(c->stream);
+    event_destroy(c->ev0);
+    event_destroy(c->ev1);
     delete c;
     e->compactor = nullptr;
   }
   if (e->read_comb) { e->read_comb->destroy(); delete e->read_comb; }
   if (e->apply_comb) { e->apply_comb->destroy(); delete e->apply_comb; }
   cudaSetDevice(e->device);
-  cudaStreamSynchronize(e->st);
+  if (e->st) cudaStreamSynchronize(e->st);
   for (rsp_snapshot* sn : e->snap_slots) delete sn;  // snapshots still held are released with their pins
-  if (e->d_snap_views) cudaFree(e->d_snap_views);
-  for (rsp_shard* s : e->slots)
-    if (s) { s->runs.clear(); delete s; }
+  cudaFree(e->d_snap_views);
+  for (rsp_shard* s : e->slots) delete s;
   e->arena.destroy();
-  e->pin_in.destroy(); e->pin_out.destroy(); e->pin_up.destroy(); e->pin_totals.destroy(); e->pin_ingest.destroy(); e->dev_up.destroy(); e->dev_tick.destroy(); e->dev_q.destroy(); e->dev_pending.destroy();
   cudaFree(e->d_shards);
   cudaFree(e->d_fast);
-  cudaEventDestroy(e->ev0); cudaEventDestroy(e->ev1); cudaEventDestroy(e->up_ev); cudaEventDestroy(e->pending_ev);
+  for (cudaEvent_t ev : {e->ev0, e->ev1, e->up_ev, e->pending_ev, e->mut_ev}) event_destroy(ev);
   e->readers.destroy();
-  cudaEventDestroy(e->mut_ev);
-  for (int k = 0; k < 3; k++) { cudaStreamDestroy(e->cs[k]); cudaEventDestroy(e->cs_done[k]); }
-  cudaStreamDestroy(e->st);
-  delete e;
+  for (int k = 0; k < 3; k++) { stream_destroy(e->cs[k]); event_destroy(e->cs_done[k]); }
+  stream_destroy(e->st);
+  delete e;  // (the scratch buffers go with it)
 }
 
 int rsp_engine_device(const rsp_engine* e) { return e->device; }
@@ -2231,7 +2176,7 @@ static int shard_open_locked(rsp_engine* e, const char* name, const rsp_shard_op
   while (ix < e->slots.size() && e->slots[ix]) ix++;
   if (ix >= e->cfg.max_shards) return RSP_BUSY;
   if (ix == e->slots.size()) e->slots.push_back(nullptr);
-  rsp_shard* s = new rsp_shard();
+  std::unique_ptr<rsp_shard> s(new rsp_shard());
   static std::atomic<u64> next_uid{1};
   s->uid = next_uid++;
   s->eng = e; s->name = name; s->index = ix;
@@ -2242,15 +2187,15 @@ static int shard_open_locked(rsp_engine* e, const char* name, const rsp_shard_op
   s->h.merge_op = s->opts.merge_op;
   s->h.merge_delim = s->opts.merge_op == RSP_MERGE_STRING_APPEND ? s->opts.merge_delim : 0u;
   s->h.live = 1;
-  alloc_memtable(e, s, 0, 0);
+  alloc_memtable(e, s.get(), 0, 0);
   UploadBatch up;
-  stage_upload(e, s, false, true, &up);
+  stage_upload(e, s.get(), false, true, &up);
   commit_uploads(e, &up);
   CUDA_OK(cudaStreamSynchronize(e->st));
   if (s->opts.merge_op == RSP_MERGE_STRING_APPEND) e->n_string_append++;
-  e->slots[ix] = s;
-  e->by_name[name] = s;
-  *out = s;
+  e->by_name[name] = s.get();
+  e->slots[ix] = s.get();
+  *out = s.release();
   return RSP_OK;
 }
 
@@ -2268,11 +2213,7 @@ static void shard_close_locked(rsp_shard* s) {
   CUDA_OK(cudaMemset(e->d_fast + s->index, 0, sizeof(ShardFast)));
   CUDA_OK(cudaMemset(e->d_fast_runs + (size_t)s->index * RSP_MAX_RUNS, 0, sizeof(ShardFast) * RSP_MAX_RUNS));
   CUDA_OK(cudaMemset(e->d_mt_filter + (size_t)s->index * MT_FILTER_WORDS, 0, MT_FILTER_WORDS * 4));
-  e->arena.release(s->h.mt_heap, s->mt_heap_bytes);
-  e->arena.release(s->h.mt_slots, s->mt_slot_bytes);
-  e->arena.release(s->h.mt_ent_off, s->mt_ent_bytes);
-  s->runs.clear();
-  delete s;
+  delete s;  // its memtable and the runs nobody else pins go back to the arena
 }
 
 int rsp_shard_open_ex(rsp_engine* e, const char* name, const rsp_shard_opts* opts, uint32_t flags, rsp_shard** out) {
@@ -2303,13 +2244,13 @@ int rsp_shard_close(rsp_shard* s) {
 static void run_key_range(rsp_engine* e, const Run& r, std::string* first, std::string* last) {
   auto key_at = [&](u32 unit, std::string* out) {
     u32 hd[4];
-    CUDA_OK(cudaMemcpy(hd, r.heap + (size_t)unit * 16, 16, cudaMemcpyDeviceToHost));
+    CUDA_OK(cudaMemcpy(hd, r.heap.get<u8>() + (size_t)unit * 16, 16, cudaMemcpyDeviceToHost));
     out->resize(hd[2]);
-    if (hd[2]) CUDA_OK(cudaMemcpy(&(*out)[0], r.heap + (size_t)unit * 16 + 16, hd[2], cudaMemcpyDeviceToHost));
+    if (hd[2]) CUDA_OK(cudaMemcpy(&(*out)[0], r.heap.get<u8>() + (size_t)unit * 16 + 16, hd[2], cudaMemcpyDeviceToHost));
   };
   u32 first_unit = 0, last_unit = 0;
-  CUDA_OK(cudaMemcpy(&first_unit, r.ent_off, 4, cudaMemcpyDeviceToHost));
-  CUDA_OK(cudaMemcpy(&last_unit, r.ent_off + (r.n_ent - 1), 4, cudaMemcpyDeviceToHost));
+  CUDA_OK(cudaMemcpy(&first_unit, r.ent_off.get<u32>(), 4, cudaMemcpyDeviceToHost));
+  CUDA_OK(cudaMemcpy(&last_unit, r.ent_off.get<u32>() + (r.n_ent - 1), 4, cudaMemcpyDeviceToHost));
   key_at(first_unit, first);
   key_at(last_unit, last);
   (void)e;
@@ -2333,64 +2274,47 @@ static void upload_staged(rsp_engine* e, void* dst, const void* src, size_t byte
 // run entry layout into a source heap, which the compaction passes (one pre-sorted source: no sort, no merge) turn into
 // the run with its restart array, block index and hash index.  Nothing reads sequence numbers inside a run against
 // anything but a snapshot bound, which sequence 0 always meets: recency between runs is the run order.  `units`: the
-// source heap's size (n + the key and value units).  On failure the work buffers go back to the arena.
+// source heap's size (n + the key and value units).  Every buffer is taken before the first copy is queued, and
+// run_jobs synchronises the stream when it fails, so the inputs go back with the stream idle.
 static std::shared_ptr<Run> build_sorted_run(rsp_engine* e, rsp_shard* s, size_t n, const uint8_t* keys,
                                              const uint64_t* koff, const uint8_t* vals, const uint64_t* voff, u64 units) {
   Arena& a = e->arena;
-  const size_t kb = std::max<size_t>(1, koff[n] - koff[0]), vb = std::max<size_t>(1, voff[n] - voff[0]);
-  const size_t ob = (n + 1) * 8, eb = n * 4, tb = (size_t)ingest_tiles((u32)n) * 4, hb = units * 16;
-  IngestArgs g{};
-  CompactPlan plan;
-  cudaEvent_t half_done[2] = {nullptr, nullptr};
-  auto release_inputs = [&] {
-    for (cudaEvent_t ev : half_done) if (ev) cudaEventDestroy(ev);
-    if (g.keys) a.release((void*)g.keys, kb);
-    if (g.vals) a.release((void*)g.vals, vb);
-    if (g.koff) a.release((void*)g.koff, ob);
-    if (g.voff) a.release((void*)g.voff, ob);
-    if (g.ent_off) a.release(g.ent_off, eb);
-    if (g.tile_sum) a.release(g.tile_sum, tb);
-    if (g.heap) a.release(g.heap, hb);
-  };
-  try {
-    for (cudaEvent_t& ev : half_done) {
-      CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
-      CUDA_OK(cudaEventRecord(ev, e->st));
-    }
-    g.n = (u32)n;
-    g.keys = (const u8*)a.alloc(kb);
-    g.vals = (const u8*)a.alloc(vb);
-    g.koff = (const u64*)a.alloc(ob);
-    g.voff = (const u64*)a.alloc(ob);
-    g.ent_off = (u32*)a.alloc(eb);
-    g.tile_sum = (u32*)a.alloc(tb);
-    g.heap = (u8*)a.alloc(hb);
-    upload_staged(e, (void*)g.keys, keys + koff[0], koff[n] - koff[0], half_done);
-    upload_staged(e, (void*)g.vals, vals + voff[0], voff[n] - voff[0], half_done);
-    upload_staged(e, (void*)g.koff, koff, ob, half_done);
-    upload_staged(e, (void*)g.voff, voff, ob, half_done);
-    launch_ingest_entries(g, e->st);
-    CUDA_OK(cudaGetLastError());
-    e->launches += 3;
-    CompactJob j;
-    memset(&j, 0, sizeof(j));
-    j.src_heap[0] = g.heap; j.src_ent_off[0] = g.ent_off; j.src_n[0] = (u32)n; j.src_is_mem[0] = 0;
-    j.n_src = 1; j.n_items = (u32)n; j.items_len = (u32)n;
-    j.merge_op = s->opts.merge_op;
-    j.merge_delim = s->h.merge_delim;
-    JobHost h{s, s->index, s->uid, true, false, 0, {}, 0, 0, 0, 0, 0};
-    alloc_job_work(a, &j, &h);
-    plan.jh.push_back(h);
-    plan.jobs.push_back(j);
-    run_jobs(e, &plan, e->st, e->ev0, e->ev1, &e->pin_totals);
-  } catch (...) {
-    cudaStreamSynchronize(e->st);
-    release_work(e, &plan);
-    release_inputs();
-    throw;
+  const size_t ob = (n + 1) * 8;
+  struct Events {
+    cudaEvent_t ev[2] = {nullptr, nullptr};
+    ~Events() { for (cudaEvent_t x : ev) if (x) cudaEventDestroy(x); }
+  } half_done;
+  for (cudaEvent_t& ev : half_done.ev) {
+    CUDA_OK(cudaEventCreateWithFlags(&ev, cudaEventDisableTiming));
+    CUDA_OK(cudaEventRecord(ev, e->st));
   }
-  release_work(e, &plan);
-  release_inputs();
+  ArenaBlock in_keys(a, std::max<size_t>(1, koff[n] - koff[0])), in_vals(a, std::max<size_t>(1, voff[n] - voff[0]));
+  ArenaBlock in_koff(a, ob), in_voff(a, ob), ent_off(a, n * 4), tile_sum(a, (size_t)ingest_tiles((u32)n) * 4);
+  ArenaBlock heap(a, units * 16);
+  IngestArgs g{};
+  g.n = (u32)n;
+  g.keys = in_keys.get<const u8>(); g.vals = in_vals.get<const u8>();
+  g.koff = in_koff.get<const u64>(); g.voff = in_voff.get<const u64>();
+  g.ent_off = ent_off.get<u32>(); g.tile_sum = tile_sum.get<u32>(); g.heap = heap.get<u8>();
+  CompactPlan plan;
+  CompactJob j;
+  memset(&j, 0, sizeof(j));
+  j.src_heap[0] = g.heap; j.src_ent_off[0] = g.ent_off; j.src_n[0] = (u32)n; j.src_is_mem[0] = 0;
+  j.n_src = 1; j.n_items = (u32)n; j.items_len = (u32)n;
+  j.merge_op = s->opts.merge_op;
+  j.merge_delim = s->h.merge_delim;
+  JobHost h{s, s->index, s->uid, true, false, 0, {}};
+  alloc_job_work(a, &j, &h);
+  plan.jh.push_back(std::move(h));
+  plan.jobs.push_back(j);
+  upload_staged(e, in_keys.get(), keys + koff[0], koff[n] - koff[0], half_done.ev);
+  upload_staged(e, in_vals.get(), vals + voff[0], voff[n] - voff[0], half_done.ev);
+  upload_staged(e, in_koff.get(), koff, ob, half_done.ev);
+  upload_staged(e, in_voff.get(), voff, ob, half_done.ev);
+  launch_ingest_entries(g, e->st);
+  CUDA_OK(cudaGetLastError());
+  e->launches += 3;
+  run_jobs(e, &plan, e->st, e->ev0, e->ev1, &e->pin_totals);
   e->last_ms["ingest"] = plan.ms;
   return plan.outs[0];
 }
@@ -2972,8 +2896,8 @@ static rsp_iter* iter_new(rsp_engine* e, rsp_shard* s, const rsp_snapshot* snap)
   if (snap) { it->pinned = snap->pinned; view_of(s, it->pinned, &v); }
   else pin_view(e, s, &it->pinned, &v);
   v.live = 1;
-  it->d_view = (ScanView*)e->arena.alloc(sizeof(ScanView));
-  CUDA_OK(cudaMemcpyAsync(it->d_view, &v, sizeof(v), cudaMemcpyHostToDevice, e->st));
+  it->view = ArenaBlock(e->arena, sizeof(ScanView));
+  CUDA_OK(cudaMemcpyAsync(it->view.get(), &v, sizeof(v), cudaMemcpyHostToDevice, e->st));
   CUDA_OK(cudaStreamSynchronize(e->st));
   return it.release();
 }
@@ -2996,13 +2920,9 @@ void rsp_iter_destroy(rsp_iter* it) {
   try {
   if (!it) return;
   rsp_engine* e = it->s->eng;
-  {
-    std::lock_guard<std::mutex> g(e->mu);
-    CUDA_OK(cudaSetDevice(e->device));
-    CUDA_OK(cudaStreamSynchronize(e->st));
-    e->arena.release(it->d_view, sizeof(ScanView));
-    it->pinned.clear();
-  }
+  std::lock_guard<std::mutex> g(e->mu);
+  CUDA_OK(cudaSetDevice(e->device));
+  CUDA_OK(cudaStreamSynchronize(e->st));  // nothing reads its view or its runs any more
   delete it;
   } catch (...) { abi_caught(); }
 }
@@ -3429,10 +3349,11 @@ int rsp_stage_build(rsp_engine* e, size_t n, const uint32_t* shard_ix, const uin
   if (!e || !out || !n) return RSP_INVALID_ARGUMENT;
   std::lock_guard<std::mutex> g(e->mu);
   CUDA_OK(cudaSetDevice(e->device));
-  rsp_staged* sg = new rsp_staged();
-  int rc = stage_build(e, n, shard_ix, blob, off, ts_ms, sg, true);
-  if (rc != RSP_OK) { delete sg; return rc; }
-  *out = sg;
+  std::unique_ptr<rsp_staged, decltype(&rsp_stage_free)> sg(new rsp_staged(), rsp_stage_free);
+  sg->eng = e;
+  int rc = stage_build(e, n, shard_ix, blob, off, ts_ms, sg.get(), true);
+  if (rc != RSP_OK) return rc;
+  *out = sg.release();
   return RSP_OK;
   } catch (...) { return abi_caught(); }
 }
